@@ -56,6 +56,9 @@ def parse():
                     help="samples in the CPU arm's batch (64 = the full C2 batch)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-profile", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (its loss and a "
+                         "fixed, seeded sample of every parameter gradient) to DIR/<name>.npy as float32")
     ap.add_argument("--overlap-chunks", type=int, default=4,
                     help="N>1: layer groups whose gradient all-reduce overlaps the backward pass")
     ap.add_argument("--sm-reserve", type=int, default=0,
@@ -95,6 +98,24 @@ def algorithmic_flops(lens, NL, H):
     return 3.0 * NL * (24.0 * H * H * T + 4.0 * H * s2)
 
 
+def dump_outputs(out_dir, loss, model, per_param=4096):
+    """loss.npy: the step's loss; grad_sample.npy: per parameter (in named_parameters order) up to
+    `per_param` gradient entries at indices drawn once from a generator seeded with 0, concatenated
+    (about 1 M float32 values for UNITER-base, well under 64 MB)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(-1).cpu().numpy())
+    gen = torch.Generator().manual_seed(0)
+    parts = []
+    for _, p in model.named_parameters():
+        if p.grad is None:
+            continue
+        g = p.grad.detach().reshape(-1)
+        idx = torch.randint(0, g.numel(), (min(per_param, g.numel()),), generator=gen)
+        parts.append(g[idx.to(g.device)].float().cpu())
+    np.save(os.path.join(out_dir, "grad_sample.npy"), torch.cat(parts).numpy())
+
+
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -102,8 +123,8 @@ def peaks():
             j = json.load(fh)
         return dict(tflops=j["bf16_tflops"], tflops_sustained=j.get("bf16_tflops_sustained"),
                     hbm_gbs=j["hbm_gbs"], source="measured (MEASURED_PEAKS.json)")
-    return dict(tflops=1590.0, tflops_sustained=1400.0, hbm_gbs=6650.0,
-                source="fallback (B200_PROFILING.md)")
+    return dict(tflops=989.0, tflops_sustained=None, hbm_gbs=3350.0,
+                source="H100 SXM data sheet, dense bf16 at 700 W (not measured)")
 
 
 class ClockSampler:
@@ -829,13 +850,17 @@ def main():
         if rank == 0:
             sampler.start()
         cpu_t = [0.0]
+        last_loss = [None]
 
         def timed_step(i):
             t0 = time.perf_counter()
-            step_resident(i)
+            last_loss[0] = step_resident(i)
             cpu_t[0] += time.perf_counter() - t0
 
         ms_total = timed(timed_step, args.steps)
+        if args.dump_outputs and rank == 0 and attempt == 0:
+            last = (args.steps - 1) % nt
+            dump_outputs(args.dump_outputs, bks[last].loss if graphed is not None else last_loss[0], model)
         cpu_enqueue_ms = cpu_t[0] / args.steps * 1e3   # host time to enqueue one step (no sync inside)
         if graphed is not None:
             launches = sum(b.launches for b in bks) // nt     # libub200 kernels inside one replay of a graph
@@ -946,24 +971,16 @@ def main():
         gemm_launches = sum(cnt_arr[i] for i in gemm_tags) // psteps
         T = sum(sum(host[i]["lens"]) for i in range(nt)) / nt
         gemm_flops = 3.0 * NL * 24.0 * ARCH["H"] ** 2 * T          # dense-projection part of §8d
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "r02_traffic.json")
-        if os.path.exists(tp):                                      # from the committed ncu capture
-            with open(tp) as fh:
-                tj = json.load(fh)
-            traffic = tj["dram_read_bytes_per_launch"] + tj["dram_write_bytes_per_launch"]
-            traffic_src = tj["source"]
         achieved = gemm_flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
-        roofline = {"bound": "tensor", "kernel": "ub::gemm_kernel (tcgen05, all 12 GEMM roles of a layer)",
+        roofline = {"bound": "tensor", "kernel": "ub::gemm_kernel (wgmma, all 12 GEMM roles of a layer)",
                     "achieved": round(achieved, 1), "peak": pk["tflops"], "unit": "TFLOP/s",
                     "frac": round(achieved / pk["tflops"], 4), "peak_source": pk["source"],
                     "launches_per_step": gemm_launches, "avg_launch_us": round(gemm_ms * 1e3 / max(1, gemm_launches), 2),
-                    "algorithmic_flops_per_step": gemm_flops, "traffic": traffic, "traffic_unit": "bytes per launch (dram read+write)",
-                    "traffic_source": traffic_src,
+                    "algorithmic_flops_per_step": gemm_flops,
                     "step_frac_of_peak": round(flops_step / (ms_step * 1e-3) / 1e12 / pk["tflops"], 4),
                     "kernel_time_share_of_step": round(gemm_ms / max(all_ms, 1e-9), 3),
                     "share_basis": "event pass: the 12 GEMM roles / all library launches, both timed launch by "
-                                   "launch (serialised); compare with the ncu launch list in profiles/",
+                                   "launch (serialised)",
                     "event_pass_ms_per_step": round(all_ms, 4)}
 
     # ---- informational: the same step followed by the fused clip + AdamW update (SURVEY.md §8f-2).
@@ -1015,7 +1032,7 @@ def main():
                                       CF["B"], sum(lens0), max(lens0)),
                        "global_batch": CF["B"] * world, "parallelism": "dp%d" % world,
                        "l2": "per-step working set (weights 0.22 GB + saved activations ~1 GB) exceeds the "
-                             "126 MB L2; no explicit flush"},
+                             "50 MB L2; no explicit flush"},
             "e2e": {"value": round(e2e_value, 1), "unit": "samples/s", "ms_per_step": round(ms_e2e, 4),
                     "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4,
                     "host_ms_per_step": round(e2e_host_ms, 3),

@@ -1,5 +1,5 @@
 /*
- * ub200.h — C ABI of the B200-native UNITER encoder hot path (libub200.so).
+ * ub200.h — C ABI of the H100-native UNITER encoder hot path (libub200.so).
  *
  * The reference (ChenRocks/UNITER) is pure Python: its "FFI" for this path is the set of
  * torch / apex / horovod library calls made by model/layer.py and model/model.py.  Each entry
@@ -40,7 +40,7 @@ enum {
 /* library identity ------------------------------------------------------------------------ */
 int ub200_version(void);                      /* MAJOR*10000 + MINOR*100 + PATCH */
 const char* ub200_last_error_string(void);    /* thread-local, never NULL */
-int ub200_device_check(void);                 /* 0 iff the current device is sm_100 (B200) */
+int ub200_device_check(void);                 /* 0 iff the current device is sm_90 (H100) */
 
 /* launch accounting / profiling (used by bench.py: "gpu_launches" and the roofline pass).
  * Tags: 0 untagged (gather / convert), 1 qkv GEMM, 2 attention fwd, 3 attn-out GEMM, 4 LN1 fwd,
@@ -58,7 +58,7 @@ int ub200_profile_enable(int on);
 int ub200_profile_collect(float* ms_per_tag, int* launches_per_tag, int ntags);
 
 /* ------------------------------------------------------------------------------------------
- * GEMM core:  D[M,N] = epilogue( sum_k A[m,k] * B[n,k] )      (tcgen05 + TMA, fp32 accumulate)
+ * GEMM core:  D[M,N] = epilogue( sum_k A[m,k] * B[n,k] )      (wgmma + TMA, fp32 accumulate)
  *
  * Replaces every nn.Linear on the path and its autograd mirror:
  *   forward  model/layer.py:76-78 (query/key/value), :112 (attention.output.dense),

@@ -7,7 +7,7 @@ product (``uniter_b200``) never does.
 
 Pinning: the reference ships NO tests or golden vectors for this path ("parity unpinned" by the
 reference's own suite).  This restatement is therefore pinned against outputs of the reference
-itself: ``tests/golden/make_goldens.py`` imports ``/root/reference/model`` (apex FusedLayerNorm
+itself: ``tests/golden/make_goldens.py`` imports the reference's ``model/`` (apex FusedLayerNorm
 shimmed to torch.nn.LayerNorm — the only apex symbol the model code uses) and stores its
 outputs; ``tests/test_oracle_golden.py`` checks this file against them.
 
@@ -16,7 +16,7 @@ reference ``UniterModel.state_dict()`` (SURVEY.md §8b), so it is independent of
 class of ours or theirs.  Autograd works through it (plain torch ops), which is how gradient
 goldens are checked.
 
-Third-party arithmetic pinned here (not in /root/reference): apex FusedLayerNorm (NGC 19.05
+Third-party arithmetic pinned here (not in the reference): apex FusedLayerNorm (NGC 19.05
 image, no version pin) = biased variance, eps inside the sqrt, fp32 statistics; Horovod 0.16.4
 allreduce = mean over ranks.
 """

@@ -16,6 +16,8 @@ Cases (SURVEY.md §8c):
            of data/itm.py:356-361) — embedding output, bit-exact row selection
   heads    VQA logits / MLM scores / ITM scores through the reference heads on top of the
            reference encoder
+  ref_heads  schema, MRFR / MRC outputs, per-task logits / losses / head gradients and hard-negative
+           train steps of the reference heads (the drop-in head tests compare against these)
 """
 import os
 import sys
@@ -28,6 +30,26 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 REF = os.environ.get("UNITER_REFERENCE", "/root/reference")
+
+
+def save_split(out_path, rec, limit=900 * 1024):
+    """np.savez_compressed into `out_path`, spilling arrays into `<name>.part<k>.npz` so that no
+    file exceeds `limit` bytes (tests/util.load_golden merges the parts)."""
+    import io
+    base = out_path[:-len(".npz")]
+    parts, cur = [], {}
+    for k, v in rec.items():
+        trial = dict(cur, **{k: v})
+        buf = io.BytesIO()
+        np.savez_compressed(buf, **trial)
+        if cur and buf.tell() > limit:
+            parts.append(cur)
+            cur = {k: v}
+        else:
+            cur = trial
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        np.savez_compressed(out_path if i == 0 else "%s.part%d.npz" % (base, i), **part)
 
 
 def import_reference():
@@ -127,8 +149,8 @@ def run_case(rm, cfg_kw, img_dim, batch, out_path, full_grads, seed=0, adversari
         if full_grads:
             rec["grad/" + name] = p.grad.numpy()
         rec["gfp/" + name] = grad_fingerprint(p.grad, name)
-    np.savez_compressed(out_path, **rec)
-    print("wrote", out_path, "%.1f KB" % (os.path.getsize(out_path) / 1024), "loss", loss.item())
+    save_split(out_path, rec)
+    print("wrote", out_path, "loss", loss.item())
     return model, state
 
 
@@ -477,6 +499,120 @@ LARGE_L1 = dict(vocab_size_or_config_json_file=28996, hidden_size=1024, num_hidd
                 hidden_dropout_prob=0.1, attention_probs_dropout_prob=0.1,
                 max_position_embeddings=512, type_vocab_size=2, initializer_range=0.02)
 
+LIB_GRAD_NAMES = ("feat_regress.net.0.weight", "feat_regress.net.2.weight", "feat_regress.bias",
+                  "region_classifier.net.0.weight", "region_classifier.net.3.weight",
+                  "region_classifier.net.3.bias", "itm_output.weight", "itm_output.bias",
+                  "uniter.pooler.dense.weight", "uniter.pooler.dense.bias",
+                  "cls.predictions.transform.dense.weight", "cls.predictions.bias",
+                  "uniter.embeddings.word_embeddings.weight", "uniter.img_embeddings.img_linear.weight",
+                  "uniter.img_embeddings.mask_embedding.weight",
+                  "uniter.encoder.layer.1.output.dense.weight")
+
+
+def heads_mrm_extra(batch):
+    """Masked regions + MRFR / MRC targets over the heads batch (model/pretrain.py:135-154, :201-229)."""
+    gen = torch.Generator().manual_seed(8)
+    img_masks = torch.rand(batch["img_feat"].shape[:2], generator=gen) < 0.4
+    for i, nb in enumerate(batch["num_bbs"]):
+        img_masks[i, nb:] = False
+    img_masks[0, 0] = True
+    img_mask_tgt = torch.zeros_like(batch["attn_masks"], dtype=torch.bool)
+    for i, tl in enumerate(batch["txt_lens"]):
+        nb = batch["num_bbs"][i]
+        img_mask_tgt[i, tl:tl + nb] = img_masks[i, :nb]
+    n = int(img_masks.sum())
+    return {"img_masks": img_masks, "img_mask_tgt": img_mask_tgt,
+            "feat_targets": batch["img_feat"][img_masks].half().float(),
+            "label_targets": torch.softmax(torch.randn(n, 11, generator=gen), -1)}
+
+
+def lib_heads_batches(use_index):
+    """CPU (16-bit-rounded) and device-agnostic batches of the library-vs-reference heads comparison."""
+    from uniter_b200.synth import synth_batch, synth_mrm
+    base = synth_batch(5, 5, 9, 4, 8, seed=17, img_dim=64, vocab_size=2000, mlm_prob=0.3)
+    mb = synth_mrm(base, mask_prob=0.3, label_dim=11, seed=3)
+    keys = [k for k, v in mb.items() if torch.is_tensor(v)]
+    if not use_index:           # the reference's own boolean-mask row selection
+        keys = [k for k in keys if k not in ("mlm_index", "mlm_targets", "mrm_index", "mrm_valid", "mrm_inv_n")]
+    cb = {k: (mb[k].half().float() if mb[k].is_floating_point() else mb[k]) for k in keys}
+    raw = {k: mb[k] for k in keys}
+    cb["targets"] = raw["targets"] = torch.tensor([1, 0, 1, 1, 0])
+    cb["ot_inputs"] = None
+    plain_c = dict(cb, img_feat=base["img_feat"].half().float())      # mlm / itm see unmasked regions
+    plain_raw = dict(raw, img_feat=base["img_feat"])
+    return cb, plain_c, raw, plain_raw
+
+
+def run_ref_heads(rm, rvqa, rpre, out_path):
+    """What the reference's own task heads compute on CPU fp32 (weights rounded to fp16), for the
+    drop-in tests of tests/test_reference_heads_gpu.py and tests/test_boundary_cpu.py:
+      config/*    the reference's model config files (JSON text)
+      keys/*      state-dict keys of the reference heads (schema the drop-in must reproduce)
+      pre/*       MRFR / MRC outputs of UniterForPretraining over the heads batch
+      lib/*       logits, per-element losses and head gradients of UniterForPretraining on the
+                  library-heads batch (the reference selects rows by the boolean masks, so the
+                  loader's index keys do not change them)
+      hn/<sf>/*   UniterForImageTextRetrievalHardNeg train step: loss and the mined rows"""
+    import model.itm as ritm
+    from uniter_b200.synth import seeded_state, synth_batch
+    cfg = rm.UniterConfig(**TINY)
+    rec = {}
+    for name in ("uniter-base.json", "uniter-large.json"):
+        with open(os.path.join(REF, "config", name)) as fh:
+            rec["config/" + name] = np.array(fh.read())
+    rec["keys/pretrain"] = np.array(sorted(rpre.UniterForPretraining(cfg, 64, 11).state_dict().keys()))
+    rec["keys/vqa"] = np.array(sorted(rvqa.UniterForVisualQuestionAnswering(cfg, 64, 17).state_dict().keys()))
+    ref = rpre.UniterForPretraining(cfg, 64, 11)
+    st = seeded_state({k: tuple(v.shape) for k, v in ref.state_dict().items()}, seed=4)
+    ref.load_state_dict({k: v.half().float() for k, v in st.items()}, strict=True)
+    ref.eval()
+    batch = synth_batch(3, 5, 9, 4, 8, seed=7, img_dim=64, vocab_size=2000, mlm_prob=0.3)
+    cb = {k: v for k, v in batch.items() if torch.is_tensor(v)}
+    cb["img_feat"] = cb["img_feat"].half().float()
+    cb["img_pos_feat"] = cb["img_pos_feat"].half().float()
+    extra = heads_mrm_extra(batch)
+    for task in ("mrfr", "mrc"):
+        with torch.no_grad():
+            rec["pre/" + task] = ref(dict(cb, **extra), task=task, compute_loss=False).numpy()
+    cbu, plain_c, _, _ = lib_heads_batches(False)
+    total = 0.0
+    for task in ("mlm", "mrfr", "mrc", "mrc-kl", "itm"):
+        bc = plain_c if task in ("mlm", "itm") else cbu
+        with torch.no_grad():
+            want = ref(bc, task=task, compute_loss=False)
+        want = want[0] if isinstance(want, tuple) else want
+        lw = ref(bc, task=task, compute_loss=True)
+        lw = lw[0] if isinstance(lw, tuple) else lw
+        rec["lib/%s/logits" % task] = want.numpy()
+        rec["lib/%s/loss" % task] = lw.detach().numpy()
+        total = total + lw.float().mean()
+    total.backward()
+    rp = dict(ref.named_parameters())
+    for name in LIB_GRAD_NAMES:
+        rec["lib/grad/%s" % name] = rp[name].grad.numpy()
+    hn = ritm.UniterForImageTextRetrievalHardNeg(cfg, 16, hard_size=3)
+    rec["keys/itm_hardneg"] = np.array(sorted(hn.state_dict().keys()))
+    st = seeded_state({k: tuple(v.shape) for k, v in hn.state_dict().items()}, seed=6)
+    for sf in ("t", "i"):
+        ref = ritm.UniterForImageTextRetrievalHardNeg(cfg, 16, hard_size=3)
+        ref.load_state_dict({k: v.half().float() for k, v in st.items()}, strict=True)
+        ref.train()
+        for _, module in ref.named_modules():
+            if isinstance(module, torch.nn.Dropout):
+                module.p = 0.0
+        cbatch, _ = hardneg_inputs(sf, seed=77)
+        cbatch["img_feat"] = cbatch["img_feat"].half().float()
+        cbatch["img_pos_feat"] = cbatch["img_pos_feat"].half().float()
+        picked = {}
+        rorig = ref._get_hard_batch
+        ref._get_hard_batch = lambda bt, sc, sfrom, _o=rorig: picked.setdefault("cpu", _o(bt, sc, sfrom))
+        rloss = ref(cbatch, sample_from=sf, compute_loss=True)
+        key = "img_feat" if sf == "t" else "input_ids"
+        rec["hn/%s/loss" % sf] = rloss.detach().numpy()
+        rec["hn/%s/rows" % sf] = picked["cpu"][key].float().numpy()
+    save_split(out_path, rec)
+    print("wrote", out_path)
+
 
 def main():
     from uniter_b200.synth import synth_batch
@@ -499,6 +635,7 @@ def main():
     run_case(rm, LARGE_L1, 2048, lg, os.path.join(HERE, "large_l1.npz"), full_grads=False)
     run_heads(rm, rvqa, rpre, os.path.join(HERE, "heads_tiny.npz"))
     run_hardneg(rm, os.path.join(HERE, "hardneg.npz"))
+    run_ref_heads(rm, rvqa, rpre, os.path.join(HERE, "ref_heads.npz"))
     run_adamw(os.path.join(HERE, "adamw.npz"))
     run_batching(os.path.join(HERE, "batching.npz"))
     run_itm_batching(os.path.join(HERE, "itm_batching.npz"))

@@ -1,4 +1,4 @@
-"""GPU: fused varlen attention (tcgen05) vs torch fp32 reference of model/layer.py:80-100."""
+"""GPU: fused varlen attention (wgmma) vs torch fp32 reference of model/layer.py:80-100."""
 import math
 
 import pytest

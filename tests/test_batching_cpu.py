@@ -54,7 +54,7 @@ def test_collates_match_reference_bit_exactly():
             ref = g["%s/%s" % (name, k)]
             assert b[k].dtype == torch.from_numpy(ref).dtype, k
             assert np.array_equal(b[k].numpy(), ref), (name, k)
-        # host-known bookkeeping added for the packed B200 path
+        # host-known bookkeeping added for the packed GPU path
         lens = [a + c for a, c in zip(b["txt_lens"], b["num_bbs"])]
         assert b["attn_masks"].sum(1).tolist() == lens
         assert b["cu_seqlens"].dtype == torch.int32

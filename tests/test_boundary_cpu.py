@@ -4,8 +4,9 @@
   * ctypes struct mirrors have the size the C compiler gives the header's structs;
   * UniterConfig / UniterModel keep the reference's constructor, parameter schema, from_pretrained
     renames and error conventions (SURVEY.md §8b-B1);
-  * the reference's own task heads accept our UniterModel when /root/reference is present
-    (construction + state-dict level; compute needs the GPU);
+  * the reference's own task heads accept our UniterModel when the reference is staged
+    (oracle/_ref), and the library's restated heads have the reference heads' state-dict schema
+    (stored from the reference) and weight tying (construction + state-dict level);
   * the product never silently falls back: forward on CPU / fp32 raises.
 """
 import ctypes as C
@@ -19,9 +20,11 @@ import tempfile
 import pytest
 import torch
 
+from oracle import ref_loader
+from tests import util
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(ROOT, "include", "ub200.h")
-REF = "/root/reference"
 
 
 @pytest.fixture(scope="module")
@@ -111,11 +114,12 @@ def test_config_matches_reference_semantics(tmp_path):
     c = UniterConfig.from_json_file(str(p))
     assert c.hidden_size == 768 and c.extra_key == 7        # every JSON key is copied (model/model.py:89-102)
     assert json.loads(c.to_json_string())["vocab_size"] == 28996
+    g = util.load_golden("ref_heads")       # the reference's own config files
     for name in ("uniter-base.json", "uniter-large.json"):
-        path = os.path.join(REF, "config", name)
-        if os.path.exists(path):
-            c = UniterConfig.from_json_file(path)
-            assert c.hidden_size == 64 * c.num_attention_heads
+        path = tmp_path / name
+        path.write_text(str(g["config/" + name]))
+        c = UniterConfig.from_json_file(str(path))
+        assert c.hidden_size == 64 * c.num_attention_heads
 
 
 def test_state_dict_schema_and_weight_decay_names():
@@ -192,31 +196,55 @@ def test_qkv_packing_survives_dtype_casts():
     assert att.key.weight.data_ptr() == att.query.weight.data_ptr() + H * H * 2
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present")
+@pytest.mark.skipif(not ref_loader.available(), reason="reference sources not staged")
 def test_reference_heads_accept_the_drop_in_model():
-    """Monkey-patch model.model.UniterModel (the INTEGRATION.md recipe) and build the reference's
-    own heads on top of it: constructor, init_weights, weight tying and state-dict keys."""
-    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-    import make_goldens
-    rm, rvqa, rpre = make_goldens.import_reference()
+    """Monkey-patch model.<head>.UniterModel (the INTEGRATION.md recipe) and build the reference's
+    own heads on top of it: constructor, init_weights, weight tying and state-dict keys (equal to
+    the reference heads over their own encoder, and to the stored schema)."""
+    rm, rvqa, rpre = ref_loader.load("model.model", "model.vqa", "model.pretrain")
     from uniter_b200.model import UniterModel
+    g = util.load_golden("ref_heads")
     orig = rm.UniterModel
     try:
         for mod in (rvqa, rpre):
             mod.UniterModel = UniterModel
-        cfg = rm.UniterConfig(**make_goldens.TINY)
+        c = util.TINY
+        cfg = rm.UniterConfig(c["vocab_size"], **{k: v for k, v in c.items() if k not in ("vocab_size", "img_dim")})
         vqa = rvqa.UniterForVisualQuestionAnswering(cfg, 64, 17)
         assert isinstance(vqa.uniter, UniterModel)
+        assert sorted(vqa.state_dict().keys()) == [str(k) for k in g["keys/vqa"]]
         pre = rpre.UniterForPretraining(cfg, 64, 11)
         assert pre.cls.predictions.decoder.weight is pre.uniter.embeddings.word_embeddings.weight
         assert pre.feat_regress.weight is pre.uniter.img_embeddings.img_linear.weight
-        ref_keys = set(rpre.UniterForPretraining.__mro__[0](cfg, 64, 11).state_dict().keys())
+        ref_keys = set(pre.state_dict().keys())
         rpre.UniterModel = orig
         want = set(rpre.UniterForPretraining(cfg, 64, 11).state_dict().keys())
         assert ref_keys == want
+        assert sorted(ref_keys) == [str(k) for k in g["keys/pretrain"]]
     finally:
         rvqa.UniterModel = orig
         rpre.UniterModel = orig
+
+
+def test_library_heads_have_the_reference_schema():
+    """uniter_b200.heads restates the reference heads: the same state-dict keys as the reference's
+    own UniterForPretraining / UniterForVisualQuestionAnswering (stored from the reference:
+    tests/golden/ref_heads.npz), the encoder's keys are their `uniter.*` keys, and the weight
+    tying holds."""
+    from uniter_b200.heads import UniterForPretraining, UniterForVisualQuestionAnswering
+    from uniter_b200.model import UniterModel
+    g = util.load_golden("ref_heads")
+    cfg = util.tiny_config()
+    vqa = UniterForVisualQuestionAnswering(cfg, 64, 17)
+    assert isinstance(vqa.uniter, UniterModel)
+    assert sorted(vqa.state_dict().keys()) == [str(k) for k in g["keys/vqa"]]
+    pre = UniterForPretraining(cfg, 64, 11)
+    assert pre.cls.predictions.decoder.weight is pre.uniter.embeddings.word_embeddings.weight
+    assert pre.feat_regress.weight is pre.uniter.img_embeddings.img_linear.weight
+    ref_keys = [str(k) for k in g["keys/pretrain"]]
+    assert sorted(pre.state_dict().keys()) == ref_keys
+    enc_keys = sorted("uniter." + k for k in UniterModel(cfg, 64).state_dict().keys())
+    assert enc_keys == [k for k in ref_keys if k.startswith("uniter.")]
 
 
 def test_prefix_pack_bookkeeping_matches_mask_derived_indices():

@@ -84,7 +84,7 @@ def test_chunk_shipping_covers_the_arena_exactly_once_and_survives_unreduced_war
     afterwards (the front-end) must tile the arena exactly once.  GraphedStep warms a step up WITHOUT the
     reducer (a capture must not communicate): the per-step counters reduce() normally clears are then
     stale and nothing may be shipped early until reset_step_state() — the regression that silently
-    removed all overlap (every N = 2 variant at 4.15 ms, profiles/r02_k_*)."""
+    removed all overlap."""
     from uniter_b200.heads import UniterForMLM
     from uniter_b200.model import UniterConfig
     from uniter_b200 import distributed as ubd

@@ -1,4 +1,4 @@
-"""GPU: tcgen05 GEMM core vs a plain torch fp32 reference of the same op (floating-point kernel:
+"""GPU: wgmma GEMM core vs a plain torch fp32 reference of the same op (floating-point kernel:
 tolerance = a few ulps of the 16-bit output type, stated per dtype)."""
 import pytest
 import torch

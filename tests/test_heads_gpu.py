@@ -1,7 +1,7 @@
 """GPU: the task heads on top of the drop-in encoder (SURVEY.md §8c G6, §8f-1).
 
 Head-level logits through OUR modules vs the goldens the reference's own heads produced
-(north star: logits within 1e-2 in fp16), the fused MLM head (tcgen05 GEMMs with n_valid /
+(north star: logits within 1e-2 in fp16), the fused MLM head (wgmma GEMMs with n_valid /
 split-K, fused cross-entropy) vs the CPU oracle including gradients, and the CE kernels alone."""
 import pytest
 import torch

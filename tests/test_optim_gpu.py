@@ -1,5 +1,5 @@
 """GPU: fused multi-tensor AdamW (ub200_grad_sumsq + ub200_adamw_step) against the reference
-optimizer's own trajectory (tests/golden/adamw.npz, produced by /root/reference/optim/adamw.py +
+optimizer's own trajectory (tests/golden/adamw.npz, produced by the reference's optim/adamw.py +
 clip_grad_norm_) and, for 16-bit models with fp32 master weights, against the CPU oracle."""
 import numpy as np
 import pytest

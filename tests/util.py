@@ -22,7 +22,13 @@ def large_batch():
 
 
 def load_golden(name):
-    return dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+    """name.npz plus its spill-over files name.part<k>.npz (no golden file exceeds 1 MB)."""
+    out = dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+    k = 1
+    while os.path.exists(os.path.join(GOLDEN, "%s.part%d.npz" % (name, k))):
+        out.update(np.load(os.path.join(GOLDEN, "%s.part%d.npz" % (name, k))))
+        k += 1
+    return out
 
 
 def state_checksum(state):

@@ -1,7 +1,7 @@
-"""Per-kernel SASS mnemonic counts of libub200.so (cuobjdump -sass): which kernels are tcgen05 / TMA / TMEM,
+"""Per-kernel SASS mnemonic counts of libub200.so (cuobjdump -sass): which kernels are wgmma (HGMMA) / TMA,
 and — for the peer exchange — which carry system-scope release / acquire accesses.
 
-    python tools/sass_summary.py > profiles/r02_sass_summary.txt
+    python tools/sass_summary.py > sass_summary.txt
 """
 import collections
 import os
@@ -11,8 +11,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "uniter_b200", "lib", "libub200.so")
-COLS = [("UTCHMMA", r"\bUTCHMMA(?!\.2CTA)"), ("UTCHMMA.2CTA", r"\bUTCHMMA\.2CTA"), ("UTMALDG", r"\bUTMALDG"),
-        ("UTMASTG", r"\bUTMASTG"), ("LDTM", r"\bLDTM"), ("STTM", r"\bSTTM"), ("UTCBAR", r"\bUTCBAR"),
+COLS = [("HGMMA", r"\bHGMMA"), ("UTMALDG", r"\bUTMALDG"), ("UTMASTG", r"\bUTMASTG"),
+        ("WARPGROUP", r"\bWARPGROUP"),
         ("MUFU.EX2", r"MUFU\.EX2"), ("MUFU.RCP", r"MUFU\.RCP"), ("MUFU.TANH", r"MUFU\.TANH"),
         ("STG.SYS", r"\bSTG\.E(\.\w+)*\.STRONG\.SYS"), ("LDG.SYS", r"\bLDG\.E(\.\w+)*\.STRONG\.SYS"),
         ("MEMBAR.SYS", r"MEMBAR\.\w+\.SYS")]
@@ -42,9 +42,9 @@ def main():
         base = re.sub(r"\(.*", "", base)
         a = agg.setdefault(base, collections.Counter())
         a.update(counts[mangled])
-    print("# SASS summary of uniter_b200/lib/libub200.so (cuobjdump -sass, sm_100a), per kernel template (all instantiations summed)")
+    print("# SASS summary of uniter_b200/lib/libub200.so (cuobjdump -sass, sm_90a), per kernel template (all instantiations summed)")
     print("# columns: instantiations | " + " | ".join(n for n, _ in COLS))
-    for base, c in sorted(agg.items(), key=lambda kv: -(kv[1]["UTCHMMA"] + kv[1]["UTCHMMA.2CTA"] + kv[1]["UTMALDG"])):
+    for base, c in sorted(agg.items(), key=lambda kv: -(kv[1]["HGMMA"] + kv[1]["UTMALDG"])):
         print("%-40s %4d | " % (base[:40], c["__n"]) + " | ".join("%5d" % c[n] for n, _ in COLS))
 
 

@@ -1,4 +1,4 @@
-"""uniter_b200 — B200-native (sm_100a) encoder hot path of ChenRocks/UNITER behind the
-reference's own `UniterModel` contract.  See DESIGN.md / INTEGRATION.md."""
+"""uniter_b200 — H100-native (sm_90a) encoder hot path of ChenRocks/UNITER behind the
+reference's own `UniterModel` contract.  See INTEGRATION.md."""
 from .model import (UniterConfig, UniterModel, UniterPreTrainedModel,  # noqa: F401
                     register_lengths)

@@ -1,6 +1,6 @@
 """ctypes binding of libub200.so — the only way Python reaches the CUDA kernels.
 
-There is deliberately no fallback: if the library is missing or the device is not sm_100 the
+There is deliberately no fallback: if the library is missing or the device is not sm_90 the
 import of the compute path raises.
 """
 import ctypes as C

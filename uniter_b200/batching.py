@@ -1,7 +1,7 @@
 """Host-side batching for the hot path (SURVEY.md §8f-3): the reference's token-bucket sampler and
 collate functions restated without their LMDB / horovod / toolz dependencies, emitting the SAME
 padded batch dict the reference models consume plus the host-known bookkeeping that lets the
-B200 path run without a single device->host read:
+GPU path run without a single device->host read:
 
 * ``TokenBucketSampler``  — data/sampler.py:17-60, same algorithm and the same use of the global
   ``random`` state (so ``random.seed(s)`` reproduces the reference's batches exactly); an explicit

@@ -22,15 +22,15 @@ static int g_sm_reserve = 0;
 int num_sms() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached[dev] = n;
   }
   int n = cached[dev] - g_sm_reserve;
-  n &= ~1;                 // CTA pairs (cta_group::2) need an even count
+  n &= ~1;                 // 2-CTA clusters need an even count
   return n < 2 ? 2 : n;
 }
 
@@ -182,8 +182,8 @@ int ub200_device_check(void) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10)
-    return ub::set_error(UB200_EUNSUPPORTED, "libub200 is built for sm_100a only; device is sm_%d%d",
+  if (major != 9 || minor != 0)
+    return ub::set_error(UB200_EUNSUPPORTED, "libub200 is built for sm_90a only; device is sm_%d%d",
                          major, minor);
   return 0;
 }

@@ -1,35 +1,40 @@
-// Fused variable-length multi-head self-attention for sm_100a (head_dim = 64).
+// Fused variable-length multi-head self-attention for sm_90a (head_dim = 64).
 //
 // Replaces model/layer.py:80-100 of the reference (transpose_for_scores, QK^T, /sqrt(d), +mask,
 // softmax, dropout, PV, permute+contiguous: ~10 launches over the padded [B,h,L,L] rectangle)
 // with ONE kernel over the packed [T, 3H] QKV matrix:
 //   * one CTA per (128-query tile, head, sequence); Q/K/V tiles are TMA'd straight out of the
 //     packed QKV buffer (column offsets 0 / H / 2H select q / k / v, +64*head selects the head);
-//   * S = Q K^T and O = P V run on tcgen05 (M=128, fp32 accumulators in TMEM);
+//   * two warpgroups, each owning 64 query rows: S = Q K^T runs on wgmma (m64n128k16, fp32
+//     accumulators in registers), O = P V on wgmma with P taken from the S registers (the fp32
+//     accumulator fragment of S is the 16-bit A fragment of P once packed);
 //   * mask-by-omission: only the S_b valid keys of the sequence take part (the reference's
 //     additive -10000 underflows to exactly 0 probability, so this is exact — SURVEY.md §8a E4);
-//   * softmax in registers, one query row per thread (TMEM lane == row), exp2 with 1/sqrt(d)
-//     folded in; probabilities are normalised and rounded to 16 bit BEFORE P.V, as the
-//     reference's fp16 softmax output is;
+//   * softmax in registers (the 4 lanes that share a row reduce with shuffles), exp2 with
+//     1/sqrt(d) folded in; probabilities are rounded to 16 bit BEFORE P.V, as the reference's
+//     fp16 softmax output is;
 //   * Philox dropout on P regenerated (not stored) by the backward kernel;
 //   * ctx is written directly in [T, H] layout; the row-wise log-sum-exp is saved for backward.
 //
 // Backward (autograd mirror of the same lines) recomputes P from Q, K and the saved LSE:
 //   dV = Pd^T dO,  dPd = dO V^T,  dS = P o (mask o dPd / keep - delta),  delta = rowsum(dO o O)
 //   dQ = scale * dS K,  dK = scale * dS^T Q
-// with all five contractions on tcgen05 from the same four TMA tiles (Q, K, V, dO); the
-// transposed operands (P^T, dS^T, V as [keys x d], ...) are expressed through MN-major UMMA
-// descriptors, nothing is transposed in memory.
+// with all five contractions on wgmma from the same four TMA tiles (Q, K, V, dO) and the Pd / dS
+// tiles the softmax threads write to shared memory; the transposed operands (P^T, dS^T, V as
+// [keys x d], ...) are read MN-major through the wgmma transpose bits, nothing is transposed in
+// memory.
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace ub {
 
 constexpr int ATT_D = 64;          // head dim (both UNITER configs)
-constexpr int ATT_BM = 128;        // query rows per CTA == TMEM lanes
+constexpr int ATT_BM = 128;        // query rows per CTA (two warpgroups of 64)
 constexpr int ATT_BN = 128;        // keys per KV block
 constexpr int ATT_TILE = ATT_BM * ATT_D * 2;   // 16 KB: one 128x64 16-bit tile
 constexpr int ATT_MAXSEQ = 512;    // dropout index pitch == max_position_embeddings
+constexpr int ATT_THREADS = 256;
 
 struct AttnParams {
   const int* cu_seqlens;   // [B+1]
@@ -47,25 +52,33 @@ struct AttnParams {
   const unsigned long long* rng_dev;   // optional device-side dropout stream offset (graph replay)
 };
 
-// Column sums over the 32 rows (= lanes) of a warp of a 32-column register block: a butterfly in
-// which every step halves the number of live columns per lane (16+8+4+2+1 = 31 shuffles); lane l
-// ends up with the total of column l and adds it to dst[l].  All 32 lanes must call it.
-__device__ __forceinline__ void warp_colsum32_atomic(const uint32_t (&r)[32], bool valid, float* dst,
+// Accumulator fragment of wgmma m64nN (per warp 16 rows): register 4*jj + 2*e + t holds row
+// (lane / 4) + 8 * e, column 8 * jj + 2 * (lane % 4) + t.
+
+// Column sums over the 16 rows of a warp of a 64-column fragment (rows with ok0 / ok1 false count
+// as zero): lanes with equal lane % 4 hold the same columns; lanes 0-3 add the totals to dst.
+__device__ __forceinline__ void frag_colsum64_atomic(const float (&d)[32], bool ok0, bool ok1, float* dst,
                                                      int lane) {
-  float v[32];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = valid ? __uint_as_float(r[i]) : 0.f;
+  for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
-  for (int off = 16; off >= 1; off >>= 1) {
-    const bool upper = (lane & off) != 0;
-#pragma unroll
-    for (int i = 0; i < off; ++i) {
-      const float send = upper ? v[i] : v[i + off];
-      const float keep = upper ? v[i + off] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+    for (int t = 0; t < 2; ++t) {
+      float x = (ok0 ? d[4 * jj + t] : 0.f) + (ok1 ? d[4 * jj + 2 + t] : 0.f);
+      x += __shfl_xor_sync(0xffffffffu, x, 4);
+      x += __shfl_xor_sync(0xffffffffu, x, 8);
+      x += __shfl_xor_sync(0xffffffffu, x, 16);
+      if (lane < 4) atomicAdd(dst + 8 * jj + 2 * lane + t, x);
     }
   }
-  atomicAdd(dst + lane, v[0]);
+}
+
+// row e of this thread's fragment pair, 64 columns, times `mul`, as 16-bit into out_row
+template <bool kBF16>
+__device__ __forceinline__ void store_frag_row(void* out_row, const float (&d)[32], int e, int q4, float mul) {
+  uint32_t* o = reinterpret_cast<uint32_t*>(out_row);
+#pragma unroll
+  for (int jj = 0; jj < 8; ++jj)
+    o[(8 * jj + 2 * q4) >> 1] = Elem<kBF16>::pack(d[4 * jj + 2 * e] * mul, d[4 * jj + 2 * e + 1] * mul);
 }
 
 // element index used to key the attention-probability dropout mask
@@ -73,23 +86,60 @@ __device__ __forceinline__ uint64_t attn_drop_group(int bh, int q, int key8) {
   return ((static_cast<uint64_t>(bh) * ATT_MAXSEQ + q) * ATT_MAXSEQ + key8) >> 3;
 }
 
-// write 8 consecutive 16-bit values (one 16-byte chunk) of row `r`, columns [col8, col8+8)
-// into a K-major SWIZZLE_128B operand made of 64-column slabs of 128 rows x 128 B.
-__device__ __forceinline__ void st_swz128(uint8_t* base, int r, int col8, uint4 v) {
-  const int slab = col8 >> 6;
-  const int chunk = (col8 & 63) >> 3;
-  uint8_t* p = base + slab * ATT_TILE + r * 128 + ((chunk ^ (r & 7)) << 4);
-  *reinterpret_cast<uint4*>(p) = v;
+// Dropout bits of 4 consecutive 8-key groups [4 jb, 4 jb + 4) of one query row, which the 4 lanes
+// of a quad share: lane q4 runs Philox once, for group 4 jb + q4, and the quad exchanges words so that
+// every lane ends up with word q4 of each group's block — the 16-bit lanes of its two keys 2 q4 and
+// 2 q4 + 1 (rand16_of(block, 2 q4 + t)).  w[t] belongs to group 4 jb + t.  All 32 lanes must call it.
+__device__ __forceinline__ void quad_drop_words(const DropoutRng& rng, int bh, int q, int key_base, int jb,
+                                                int lane, uint32_t (&w)[4]) {
+  const int q4 = lane & 3;
+  const uint4 r = rng.draw8(attn_drop_group(bh, q, key_base + 8 * (4 * jb + q4)));
+  uint32_t got[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    // round k: every lane sends word (q4 - k) & 3 and reads lane (q4 + k) & 3 of its quad, which
+    // sent exactly word q4 of group 4 jb + ((q4 + k) & 3)
+    const int sw = (q4 - k) & 3;
+    const uint32_t v = sw == 0 ? r.x : (sw == 1 ? r.y : (sw == 2 ? r.z : r.w));
+    got[k] = __shfl_sync(0xffffffffu, v, (lane & ~3) | ((q4 + k) & 3));
+  }
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const int k = (t - q4) & 3;
+    w[t] = k == 0 ? got[0] : (k == 1 ? got[1] : (k == 2 ? got[2] : got[3]));
+  }
 }
 
-// kSingle: every sequence of the launch fits one 128-key block (max_seqlen <= 128: all of C2 / C4 / C5).
-// The kernel is latency bound (TMA -> MMA -> TMEM -> exp -> smem -> MMA -> TMEM -> store, one chain
-// per CTA), so what matters is how many CTAs an SM can hold.  With one key block Q and K are dead
-// once S = Q K^T has completed and S is dead once P has been extracted, so P overwrites the Q|K
-// tiles and O overwrites the S columns: 48 KB smem + 128 TMEM columns per CTA -> 4 CTAs / SM
-// instead of 2 (80 KB, 256 columns).
-template <bool kBF16, bool kSingle>
-__global__ void __launch_bounds__(128, kSingle ? 4 : 2)
+__device__ __forceinline__ uint32_t rand16_half(uint32_t w, int t) { return t ? (w >> 16) : (w & 0xFFFFu); }
+
+// write two consecutive 16-bit values (one 32-bit word) of row `r`, columns [col, col+2), into a
+// K-major SWIZZLE_128B operand made of 64-column slabs of 128 rows x 128 B.
+__device__ __forceinline__ void st_swz128_u32(uint8_t* base, int r, int col, uint32_t v) {
+  const int slab = col >> 6;
+  const int chunk = (col & 63) >> 3;
+  uint8_t* p = base + slab * ATT_TILE + r * 128 + ((chunk ^ (r & 7)) << 4) + (col & 7) * 2;
+  *reinterpret_cast<uint32_t*>(p) = v;
+}
+
+// S[64 rows of warpgroup wg, 128 keys] = A[rows] . B[keys]^T, both K-major 128 x 64 tiles
+template <bool kBF16>
+__device__ __forceinline__ void qk_block(float (&s)[64], uint32_t sA, uint32_t sB, int wg) {
+#pragma unroll
+  for (int k = 0; k < ATT_D / 16; ++k)
+    Wgmma<128, kBF16, 0, 0>::ss(s, gmma_desc(sA + wg * (64 * 128) + k * 32, 16, 1024),
+                                gmma_desc(sB + k * 32, 16, 1024), k != 0);
+}
+
+// Short sequences: head-pair packing.  A sequence of <= 64 tokens fills only half of the 128-row
+// tile, so one CTA carries TWO heads: rows 0-63 (warpgroup 0) = head h0, rows 64-127 (warpgroup 1)
+// = head h0+1, keys likewise.  S = Q K^T over the 128 stacked keys is block diagonal in what
+// matters; the off-diagonal blocks of P are zeros so that O = P V stays one 128-key contraction.
+// Two CTAs per SM cap the kernel at 128 registers, at which ptxas serialises its wgmma chains
+// (C7512, S = 64 and O = 32 fp32 registers live).  Measured at C2 on H100 (profiles/
+// h100_c2_bench.jsonl, breakdown.attn_fwd): 0.38 ms per step at two CTAs per SM against 0.49 ms at
+// one CTA with unserialised wgmma — the second CTA hides more latency than the pipelining gains.
+template <bool kBF16>
+__global__ void __launch_bounds__(ATT_THREADS, 2)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmQKV64,
                 const AttnParams p) {
   pdl_launch_dependents();
@@ -97,11 +147,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
   const int b = blockIdx.z, qt = blockIdx.x;
   const int seq0 = p.cu_seqlens[b];
   const int S = p.cu_seqlens[b + 1] - seq0;
-  if (qt * ATT_BM >= S) return;  // whole CTA exits together, before any barrier / TMEM use
-  // Head-pair packing: a sequence of <= 64 tokens fills only half of the 128-row MMA tile, so
-  // one CTA carries TWO heads: rows 0-63 = head h0, rows 64-127 = head h0+1, keys likewise.
-  // S = Q K^T over the 128 stacked keys is block diagonal in what matters; the off-diagonal
-  // blocks of P are written as zeros so that O = P V stays one 128-key contraction.
+  if (qt * ATT_BM >= S) return;  // whole CTA exits together, before any barrier use
   const bool pair = (S <= 64) && ((p.nheads & 1) == 0);
   if (pair && static_cast<int>(blockIdx.y) >= p.nheads / 2) return;
   const int h0 = pair ? 2 * blockIdx.y : blockIdx.y;
@@ -110,52 +156,44 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
   if (p.drop_thr16) rng_add_dev_offset(p.rng_dev, rs0, rs1);
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // kSingle requests no alignment slack (4 CTAs must fit an SM): the dynamic window starts 1024-aligned
-  uint8_t* smem = smem_raw + (kSingle ? 0u : ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
-  if (kSingle && (smem_u32(smem_raw) & 1023u) != 0) __trap();
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;
   uint8_t* sK = smem + ATT_TILE;
   uint8_t* sV = smem + 2 * ATT_TILE;
-  uint8_t* sP = kSingle ? smem : smem + 3 * ATT_TILE;  // 2 slabs (kSingle: over the dead Q | K tiles)
-  uint64_t* bar_load = reinterpret_cast<uint64_t*>(smem + (kSingle ? 3 : 5) * ATT_TILE);
-  uint64_t* bar_mma = bar_load + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_mma + 1);
+  uint64_t* bar_load = reinterpret_cast<uint64_t*>(smem + 3 * ATT_TILE);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2, q4 = lane & 3;
   if (tid == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmQKV64);
     mbar_init(bar_load, 1);
-    mbar_init(bar_mma, 1);
     fence_barrier_init();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, kSingle ? 128 : 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tS = tmem;                        // 128 fp32 columns
-  const uint32_t tO = kSingle ? tmem : tmem + 128;   // 64 fp32 columns (kSingle: over the dead S columns)
-  const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
 
-  // this thread's query row: (head, position in the sequence, first key column of its block)
-  const int half = pair ? (tid >> 6) : 0;
+  // this thread's two query rows (tile rows r_loc[e]), their head and key block
+  const int half = pair ? wg : 0;
   const int head = h0 + half;
-  const int qrow = pair ? (tid & 63) : qt * ATT_BM + tid;
   const int kcol0 = half * 64;
-  const bool q_ok = qrow < S;
+  int qrow[2];
+  bool q_ok[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const int r_loc = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * e;
+    qrow[e] = pair ? (r_loc & 63) : qt * ATT_BM + r_loc;
+    q_ok[e] = qrow[e] < S;
+  }
   const int bh = b * p.nheads + head;
   const float c = p.scale * 1.4426950408889634f;  // scale * log2(e)
-  uint32_t ph_load = 0, ph_mma = 0;
+  const uint32_t uQ = smem_u32(sQ), uK = smem_u32(sK), uV = smem_u32(sV);
+  uint32_t ph_load = 0;
+  float s[64];
 
   // ---------------------------------------------------------------- sweep 1: row max
-  float m = -INFINITY, l = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   for (int j = 0; j < nkv; ++j) {
     const int kv_len = pair ? S : min(ATT_BN, S - j * ATT_BN);
-    const int n_pad = pair ? ATT_BN : ((kv_len + 15) & ~15);
     if (tid == 0) {
       if (pair) {
         mbar_expect_tx(bar_load, 3 * ATT_TILE);
@@ -172,174 +210,117 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
         tma_load_2d(sK, &tmQKV, bar_load, p.H + head * ATT_D, seq0 + j * ATT_BN);
         if (with_v) tma_load_2d(sV, &tmQKV, bar_load, 2 * p.H + head * ATT_D, seq0 + j * ATT_BN);
       }
-      mbar_wait(bar_load, ph_load);
-      tc_fence_after();
-      const uint32_t idesc = umma_idesc(kBF16 ? 1 : 0, 0, 0, ATT_BM, n_pad);
-#pragma unroll
-      for (int k = 0; k < ATT_D / 16; ++k)
-        umma_ss(tS, umma_smem_desc(smem_u32(sQ) + k * 32, 16, 1024),
-                umma_smem_desc(smem_u32(sK) + k * 32, 16, 1024), idesc, k != 0);
-      umma_commit(bar_mma);
     }
+    mbar_wait(bar_load, ph_load);
     ph_load ^= 1;
-    mbar_wait(bar_mma, ph_mma);
-    ph_mma ^= 1;
-    tc_fence_after();
-    for (int cc = 0; cc * 32 < kv_len; ++cc) {
-      uint32_t r[32];
-      tmem_ld32(tS + lane_off + kcol0 + cc * 32, r);
-      tmem_ld_wait();
-      if ((cc + 1) * 32 <= kv_len) {
+    wgmma_fence();
+    qk_block<kBF16>(s, uQ, uK, wg);
+    wgmma_commit();
+    wgmma_wait<0>();
 #pragma unroll
-        for (int i = 0; i < 32; ++i) m = fmaxf(m, __uint_as_float(r[i]));
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i)
-          if (cc * 32 + i < kv_len) m = fmaxf(m, __uint_as_float(r[i]));
-      }
+    for (int i = 0; i < 64; ++i) {
+      const int key = 8 * (i >> 2) + 2 * q4 + (i & 1) - kcol0;
+      if (key >= 0 && key < kv_len) m[(i >> 1) & 1] = fmaxf(m[(i >> 1) & 1], s[i]);
     }
-    if (nkv > 1) {  // S (TMEM) and sK are about to be overwritten
-      tc_fence_before();
-      __syncthreads();
-      tc_fence_after();
-    }
+    if (nkv > 1) __syncthreads();   // sK is about to be overwritten
   }
-  const float mc = m * c;
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    m[e] = fmaxf(m[e], __shfl_xor_sync(0xffffffffu, m[e], 1));
+    m[e] = fmaxf(m[e], __shfl_xor_sync(0xffffffffu, m[e], 2));
+  }
+  const float mc[2] = {m[0] * c, m[1] * c};
 
   // ---------------------------------------------------------------- sweep 2: P and O = P V
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
   for (int j = 0; j < nkv; ++j) {
     const int kv_len = pair ? S : min(ATT_BN, S - j * ATT_BN);
-    const int n_pad = pair ? ATT_BN : ((kv_len + 15) & ~15);
     if (nkv > 1) {
       if (tid == 0) {
         mbar_expect_tx(bar_load, 2 * ATT_TILE);
         tma_load_2d(sK, &tmQKV, bar_load, p.H + head * ATT_D, seq0 + j * ATT_BN);
         tma_load_2d(sV, &tmQKV, bar_load, 2 * p.H + head * ATT_D, seq0 + j * ATT_BN);
-        mbar_wait(bar_load, ph_load);
-        tc_fence_after();
-        const uint32_t idesc = umma_idesc(kBF16 ? 1 : 0, 0, 0, ATT_BM, n_pad);
-#pragma unroll
-        for (int k = 0; k < ATT_D / 16; ++k)
-          umma_ss(tS, umma_smem_desc(smem_u32(sQ) + k * 32, 16, 1024),
-                  umma_smem_desc(smem_u32(sK) + k * 32, 16, 1024), idesc, k != 0);
-        umma_commit(bar_mma);
       }
+      mbar_wait(bar_load, ph_load);
       ph_load ^= 1;
-      mbar_wait(bar_mma, ph_mma);
-      ph_mma ^= 1;
-      tc_fence_after();
+      wgmma_fence();
+      qk_block<kBF16>(s, uQ, uK, wg);
+      wgmma_commit();
+      wgmma_wait<0>();
     }
-    // probabilities -> 16-bit -> swizzled smem (A operand of P.V)
-    const int own_pad = pair ? 64 : n_pad;     // columns of this row's own block
-    for (int cc = 0; cc * 32 < own_pad; ++cc) {
-      uint32_t r[32];
-      tmem_ld32(tS + lane_off + kcol0 + cc * 32, r);
-      tmem_ld_wait();
+    // probabilities in place of the scores: unnormalised exp(scale*(s - max)) in (0, 1]; O is
+    // divided by the row sum at the end (the 1/l factor commutes with dropout and with P.V)
+    DropoutRng rng;
+    rng.k0 = p.seed_lo; rng.k1 = p.seed_hi; rng.s0 = rs0; rng.s1 = rs1;
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const int key0 = cc * 32 + g * 8;  // within this row's key block
-        if (key0 >= own_pad) break;
-        float pv[8];
+    for (int jb = 0; jb < 4; ++jb) {
+      uint32_t dw[2][4];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float sc = __uint_as_float(r[g * 8 + i]);
-          // unnormalised probability exp(scale*(s - max)) in (0, 1]; O is divided by the row sum
-          // at the end (the 1/l factor commutes with dropout and with P.V)
-          pv[i] = (key0 + i < kv_len) ? ex2_approx(fmaf(sc, c, -mc)) : 0.f;
-          l += pv[i];
-        }
-        if (p.drop_thr16) {
-          DropoutRng rng;
-          rng.k0 = p.seed_lo; rng.k1 = p.seed_hi; rng.s0 = rs0; rng.s1 = rs1;
-          const uint4 rnd = rng.draw8(attn_drop_group(bh, qrow, j * ATT_BN + key0));
+      for (int e = 0; e < 2; ++e)
+        if (p.drop_thr16) quad_drop_words(rng, bh, qrow[e], j * ATT_BN - kcol0, jb, lane, dw[e]);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            // round P to 16 bit first (reference: softmax output is fp16, then dropout)
-            const float pr = Elem<kBF16>::to_f(Elem<kBF16>::from_f(pv[i]));
-            pv[i] = (rand16_of(rnd, i) < p.drop_thr16) ? 0.f : pr * p.drop_inv_keep;
+      for (int jq = 0; jq < 4; ++jq) {
+        const int jj = 4 * jb + jq;
+        const int key0 = 8 * jj - kcol0;           // first key of this 8-key group in the KV block
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+#pragma unroll
+          for (int t = 0; t < 2; ++t) {
+            const int i = 4 * jj + 2 * e + t;
+            const int key = key0 + 2 * q4 + t;
+            float pv = (key >= 0 && key < kv_len) ? ex2_approx(fmaf(s[i], c, -mc[e])) : 0.f;
+            l[e] += pv;
+            if (p.drop_thr16) {
+              // round P to 16 bit first (reference: softmax output is fp16, then dropout)
+              const float pr = Elem<kBF16>::to_f(Elem<kBF16>::from_f(pv));
+              pv = (rand16_half(dw[e][jq], t) < p.drop_thr16) ? 0.f : pr * p.drop_inv_keep;
+            }
+            s[i] = pv;
           }
         }
-        uint4 u;
-        u.x = Elem<kBF16>::pack(pv[0], pv[1]);
-        u.y = Elem<kBF16>::pack(pv[2], pv[3]);
-        u.z = Elem<kBF16>::pack(pv[4], pv[5]);
-        u.w = Elem<kBF16>::pack(pv[6], pv[7]);
-        st_swz128(sP, tid, kcol0 + key0, u);
       }
     }
-    if (pair) {   // the other head's 64 key columns of this row: exact zeros
+    wgmma_fence();
 #pragma unroll
-      for (int g = 0; g < 8; ++g) st_swz128(sP, tid, (64 - kcol0) + g * 8, make_uint4(0, 0, 0, 0));
+    for (int kk = 0; kk < ATT_BN / 16; ++kk) {
+      const uint32_t a[4] = {Elem<kBF16>::pack(s[8 * kk + 0], s[8 * kk + 1]),
+                             Elem<kBF16>::pack(s[8 * kk + 2], s[8 * kk + 3]),
+                             Elem<kBF16>::pack(s[8 * kk + 4], s[8 * kk + 5]),
+                             Elem<kBF16>::pack(s[8 * kk + 6], s[8 * kk + 7])};
+      Wgmma<64, kBF16, 0, 1>::rs(o, a, gmma_desc(uV + kk * 2048, 8192, 1024), (j | kk) != 0);
     }
-    fence_proxy_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      const uint32_t idesc = umma_idesc(kBF16 ? 1 : 0, 0, 1, ATT_BM, ATT_D);
-      const int nk16 = n_pad >> 4;
-      for (int kk = 0; kk < nk16; ++kk) {
-        const uint32_t a = smem_u32(sP) + (kk >> 2) * ATT_TILE + (kk & 3) * 32;
-        const uint32_t bb = smem_u32(sV) + kk * 2048;
-        umma_ss(tO, umma_smem_desc(a, 16, 1024), umma_smem_desc(bb, 8192, 1024), idesc,
-                (j | kk) != 0);
-      }
-      umma_commit(bar_mma);
-    }
-    mbar_wait(bar_mma, ph_mma);
-    ph_mma ^= 1;
-    tc_fence_after();
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (nkv > 1) __syncthreads();   // sK / sV are about to be overwritten
   }
 
   // ---------------------------------------------------------------- epilogue: O / l -> ctx[T, H]
-  const float inv_l = 1.f / l;
-  if (q_ok) p.lse[static_cast<size_t>(head) * p.T + seq0 + qrow] = m * p.scale + logf(l);
-  {
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    l[e] += __shfl_xor_sync(0xffffffffu, l[e], 1);
+    l[e] += __shfl_xor_sync(0xffffffffu, l[e], 2);
+    if (!q_ok[e]) continue;
+    if (q4 == 0) p.lse[static_cast<size_t>(head) * p.T + seq0 + qrow[e]] = m[e] * p.scale + logf(l[e]);
     typename Elem<kBF16>::T* out = reinterpret_cast<typename Elem<kBF16>::T*>(p.ctx) +
-                                   static_cast<size_t>(seq0 + qrow) * p.H + head * ATT_D;
-#pragma unroll
-    for (int cc = 0; cc < 2; ++cc) {
-      uint32_t r[32];
-      tmem_ld32(tO + lane_off + cc * 32, r);
-      tmem_ld_wait();
-      if (q_ok) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 u;
-          u.x = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 0]) * inv_l, __uint_as_float(r[g * 8 + 1]) * inv_l);
-          u.y = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 2]) * inv_l, __uint_as_float(r[g * 8 + 3]) * inv_l);
-          u.z = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 4]) * inv_l, __uint_as_float(r[g * 8 + 5]) * inv_l);
-          u.w = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 6]) * inv_l, __uint_as_float(r[g * 8 + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(out + cc * 32 + g * 8) = u;
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, kSingle ? 128 : 256);
+                                   static_cast<size_t>(seq0 + qrow[e]) * p.H + head * ATT_D;
+    store_frag_row<kBF16>(out, o, e, q4, 1.f / l[e]);
   }
 }
 
-constexpr int ATT_FWD_SMEM = 5 * ATT_TILE + 64 + 1024;
-constexpr int ATT_FWD_SMEM_SINGLE = 3 * ATT_TILE + 64;
+constexpr int ATT_FWD_SMEM = 3 * ATT_TILE + 64 + 1024;
 
 // =====================================================================================
 // Backward.  One CTA per (128-key block j, head, sequence); loops over 128-query blocks i.
-//   TMEM (512 cols): S[128] | dP[128] | dV[64] | dK[64] | dQ[64]
 //   smem: Q_i, dO_i, K_j, V_j (TMA, 128B swizzle) + Pd and dS written by the softmax threads
 //   (row = query, 64-key slabs) and consumed both K-major (dQ = dS K) and MN-major
-//   (dV = Pd^T dO, dK = dS^T Q) by tcgen05.
+//   (dV = Pd^T dO, dK = dS^T Q) by wgmma.  Warpgroup wg owns query rows [64 wg, +64) of S / dP /
+//   dQ and key rows [64 wg, +64) of dK / dV (the accumulators of dK / dV live across the loop).
 // dQ of a sequence longer than one key block is accumulated with fp32 atomics in `dq_accum`.
 // =====================================================================================
-// kSingle (max_seqlen <= 128, one query block and one key block per sequence): V is dead after
-// dP = dO V^T and S / dP are dead once P / dS have been extracted, so the first P slab overwrites the
-// V tile and dV | dK | dQ overwrite the S | dP columns: 112 KB smem + 256 TMEM columns -> 2 CTAs / SM
-// (128 registers x 256 threads x 2 = the whole register file) instead of 1.
-template <bool kBF16, bool kSingle>
-__global__ void __launch_bounds__(256, kSingle ? 2 : 1)
+template <bool kBF16>
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
                 const __grid_constant__ CUtensorMap tmQKV64, const __grid_constant__ CUtensorMap tmDO64,
                 const AttnParams p, float* dq_accum) {
@@ -360,58 +341,49 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
   uint32_t rs0 = p.stream_lo, rs1 = p.stream_hi;
   if (p.drop_thr16) rng_add_dev_offset(p.rng_dev, rs0, rs1);
   const int kv_len = pair ? S : min(ATT_BN, S - j * ATT_BN);
-  const int n_pad = pair ? ATT_BN : ((kv_len + 15) & ~15);
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + (kSingle ? 0u : ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
-  if (kSingle && (smem_u32(smem_raw) & 1023u) != 0) __trap();
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;
   uint8_t* sdO = smem + ATT_TILE;
   uint8_t* sK = smem + 2 * ATT_TILE;
   uint8_t* sV = smem + 3 * ATT_TILE;
-  uint8_t* sP = smem + (kSingle ? 3 : 4) * ATT_TILE;   // 2 slabs (kSingle: slab 0 over the dead V tile)
-  uint8_t* sDS = smem + (kSingle ? 5 : 6) * ATT_TILE;  // 2 slabs
-  uint64_t* bar_load = reinterpret_cast<uint64_t*>(smem + (kSingle ? 7 : 8) * ATT_TILE);
-  uint64_t* bar_mma = bar_load + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar_mma + 1);
+  uint8_t* sP = smem + 4 * ATT_TILE;    // 2 slabs
+  uint8_t* sDS = smem + 6 * ATT_TILE;   // 2 slabs
+  uint64_t* bar_load = reinterpret_cast<uint64_t*>(smem + 8 * ATT_TILE);
 
-  // 256 threads: thread pair (row, chalf) — both own TMEM lane `row`, each handles half of the
-  // 32-column blocks (twice the warps per SM and half the serial softmax work per thread)
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int row_t = tid & 127;
-  const int chalf = tid >> 7;
-  const int half = pair ? (row_t >> 6) : 0;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2, q4 = lane & 3;
+  const int half = pair ? wg : 0;
   const int head = h0 + half;
   const int kcol0 = half * 64;
   if (tid == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmDO);
     mbar_init(bar_load, 1);
-    mbar_init(bar_mma, 1);
     fence_barrier_init();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, kSingle ? 256 : 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tS = tmem, tP = tmem + 128;
-  const uint32_t tdV = tmem + (kSingle ? 0 : 256), tdK = tmem + (kSingle ? 64 : 320),
-                 tdQ = tmem + (kSingle ? 128 : 384);
-  const uint32_t lane_off = static_cast<uint32_t>((warp & 3) * 32) << 16;
+  int r_loc[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e) r_loc[e] = 64 * wg + 16 * (warp & 3) + (lane >> 2) + 8 * e;
   const int bh = b * p.nheads + head;
   const float c = p.scale * 1.4426950408889634f;
-  const uint32_t fmt = kBF16 ? 1 : 0;
-  uint32_t ph_load = 0, ph_mma = 0;
+  const uint32_t uQ = smem_u32(sQ), udO = smem_u32(sdO), uK = smem_u32(sK), uV = smem_u32(sV);
+  const uint32_t uP = smem_u32(sP), uDS = smem_u32(sDS);
+  uint32_t ph_load = 0;
+  float dv[32], dk[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
 
   for (int i = 0; i < nq; ++i) {
-    const int q_len = min(ATT_BM, S - i * ATT_BM);
-    const int q_pad = pair ? ATT_BM : ((q_len + 15) & ~15);
-    const int qrow = pair ? (row_t & 63) : i * ATT_BM + row_t;
-    const bool q_ok = qrow < S;
+    int qrow[2];
+    bool q_ok[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      qrow[e] = pair ? (r_loc[e] & 63) : i * ATT_BM + r_loc[e];
+      q_ok[e] = qrow[e] < S;
+    }
     if (tid == 0) {
       if (pair) {
         mbar_expect_tx(bar_load, 4 * ATT_TILE);
@@ -432,196 +404,142 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant
           tma_load_2d(sV, &tmQKV, bar_load, 2 * p.H + head * ATT_D, seq0 + j * ATT_BN);
         }
       }
-      mbar_wait(bar_load, ph_load);
-      tc_fence_after();
-      const uint32_t idesc = umma_idesc(fmt, 0, 0, ATT_BM, n_pad);
-#pragma unroll
-      for (int k = 0; k < ATT_D / 16; ++k)   // S = Q K^T
-        umma_ss(tS, umma_smem_desc(smem_u32(sQ) + k * 32, 16, 1024),
-                umma_smem_desc(smem_u32(sK) + k * 32, 16, 1024), idesc, k != 0);
-#pragma unroll
-      for (int k = 0; k < ATT_D / 16; ++k)   // dPd = dO V^T
-        umma_ss(tP, umma_smem_desc(smem_u32(sdO) + k * 32, 16, 1024),
-                umma_smem_desc(smem_u32(sV) + k * 32, 16, 1024), idesc, k != 0);
-      umma_commit(bar_mma);
     }
+
+    // delta = rowsum(dO o O) and the saved log-sum-exp, straight from global (overlaps the loads);
+    // each of the 4 lanes of a row takes 16 of its 64 columns
+    float delta[2], lse2[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float d = 0.f;
+      lse2[e] = 0.f;
+      if (q_ok[e]) {
+        const size_t off = static_cast<size_t>(seq0 + qrow[e]) * p.H + head * ATT_D + 16 * q4;
+        const uint4* g_do = reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.dctx) + off);
+        const uint4* g_o = reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.ctx) + off);
+#pragma unroll
+        for (int v = 0; v < 2; ++v) {
+          const uint4 a = __ldg(g_do + v), o = __ldg(g_o + v);
+          float2 x, y;
+          x = Elem<kBF16>::unpack(a.x); y = Elem<kBF16>::unpack(o.x); d += x.x * y.x + x.y * y.y;
+          x = Elem<kBF16>::unpack(a.y); y = Elem<kBF16>::unpack(o.y); d += x.x * y.x + x.y * y.y;
+          x = Elem<kBF16>::unpack(a.z); y = Elem<kBF16>::unpack(o.z); d += x.x * y.x + x.y * y.y;
+          x = Elem<kBF16>::unpack(a.w); y = Elem<kBF16>::unpack(o.w); d += x.x * y.x + x.y * y.y;
+        }
+        lse2[e] = p.lse[static_cast<size_t>(head) * p.T + seq0 + qrow[e]] * 1.4426950408889634f;
+      }
+      d += __shfl_xor_sync(0xffffffffu, d, 1);
+      d += __shfl_xor_sync(0xffffffffu, d, 2);
+      delta[e] = d;
+    }
+
+    mbar_wait(bar_load, ph_load);
     ph_load ^= 1;
+    float s[64], dp[64];
+    wgmma_fence();
+    qk_block<kBF16>(s, uQ, uK, wg);     // S = Q K^T
+    qk_block<kBF16>(dp, udO, uV, wg);   // dPd = dO V^T
+    wgmma_commit();
+    wgmma_wait<0>();
 
-    // delta = rowsum(dO o O) and the saved log-sum-exp, straight from global (overlaps the MMAs)
-    float delta = 0.f, lse2 = 0.f;
-    if (q_ok) {
-      const size_t off = static_cast<size_t>(seq0 + qrow) * p.H + head * ATT_D;
-      const uint4* g_do = reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.dctx) + off);
-      const uint4* g_o = reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.ctx) + off);
+    DropoutRng rng;
+    rng.k0 = p.seed_lo; rng.k1 = p.seed_hi; rng.s0 = rs0; rng.s1 = rs1;
 #pragma unroll
-      for (int v = 0; v < 8; ++v) {
-        const uint4 a = __ldg(g_do + v), o = __ldg(g_o + v);
-        float2 x, y;
-        x = Elem<kBF16>::unpack(a.x); y = Elem<kBF16>::unpack(o.x); delta += x.x * y.x + x.y * y.y;
-        x = Elem<kBF16>::unpack(a.y); y = Elem<kBF16>::unpack(o.y); delta += x.x * y.x + x.y * y.y;
-        x = Elem<kBF16>::unpack(a.z); y = Elem<kBF16>::unpack(o.z); delta += x.x * y.x + x.y * y.y;
-        x = Elem<kBF16>::unpack(a.w); y = Elem<kBF16>::unpack(o.w); delta += x.x * y.x + x.y * y.y;
-      }
-      lse2 = p.lse[static_cast<size_t>(head) * p.T + seq0 + qrow] * 1.4426950408889634f;
-    }
-
-    mbar_wait(bar_mma, ph_mma);
-    ph_mma ^= 1;
-    tc_fence_after();
-
-    // 32-column blocks of this thread: pair mode -> one block of the row's own 64 columns (and
-    // zero-fill of the matching block of the other head); else two of the up to four blocks.
-    const int cc_begin = pair ? (half * 2 + chalf) : chalf * 2;
-    const int cc_end = pair ? cc_begin + 1 : chalf * 2 + 2;
-    for (int cc = cc_begin; cc < cc_end && cc * 32 < n_pad; ++cc) {
-      uint32_t rs[32], rp[32];
-      tmem_ld32(tS + lane_off + cc * 32, rs);
-      tmem_ld32(tP + lane_off + cc * 32, rp);
-      tmem_ld_wait();
+    for (int jb = 0; jb < 4; ++jb) {
+      uint32_t dw[2][4];
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const int col0 = cc * 32 + g * 8;          // column in the 128-wide tile
-        if (col0 >= n_pad) break;
-        const int key0 = col0 - kcol0;             // key index inside this KV block
-        float pd[8], ds[8];
-        uint4 rnd = make_uint4(0, 0, 0, 0);
-        if (p.drop_thr16) {
-          DropoutRng rng;
-          rng.k0 = p.seed_lo; rng.k1 = p.seed_hi; rng.s0 = rs0; rng.s1 = rs1;
-          rnd = rng.draw8(attn_drop_group(bh, qrow, j * ATT_BN + key0));
-        }
+      for (int e = 0; e < 2; ++e)
+        if (p.drop_thr16) quad_drop_words(rng, bh, qrow[e], j * ATT_BN - kcol0, jb, lane, dw[e]);
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const bool ok = q_ok && (key0 + e < kv_len);
-          float pr = ok ? ex2_approx(fmaf(__uint_as_float(rs[g * 8 + e]), c, -lse2)) : 0.f;
-          pr = Elem<kBF16>::to_f(Elem<kBF16>::from_f(pr));   // P as the forward rounded it
-          float dp = __uint_as_float(rp[g * 8 + e]);
-          float pdv = pr;
-          if (p.drop_thr16) {
-            const bool drop = rand16_of(rnd, e) < p.drop_thr16;
-            pdv = drop ? 0.f : pr * p.drop_inv_keep;
-            dp = drop ? 0.f : dp * p.drop_inv_keep;
+      for (int jq = 0; jq < 4; ++jq) {
+        const int jj = 4 * jb + jq;
+        const int key0 = 8 * jj - kcol0;            // first key of this 8-key group in the KV block
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float pd[2], ds[2];
+#pragma unroll
+          for (int t = 0; t < 2; ++t) {
+            const int idx = 4 * jj + 2 * e + t;
+            const int key = key0 + 2 * q4 + t;
+            const bool ok = q_ok[e] && key >= 0 && key < kv_len;
+            float pr = ok ? ex2_approx(fmaf(s[idx], c, -lse2[e])) : 0.f;
+            pr = Elem<kBF16>::to_f(Elem<kBF16>::from_f(pr));   // P as the forward rounded it
+            float dpv = dp[idx];
+            float pdv = pr;
+            if (p.drop_thr16) {
+              const bool drop = rand16_half(dw[e][jq], t) < p.drop_thr16;
+              pdv = drop ? 0.f : pr * p.drop_inv_keep;
+              dpv = drop ? 0.f : dpv * p.drop_inv_keep;
+            }
+            pd[t] = pdv;
+            ds[t] = ok ? pr * (dpv - delta[e]) * p.scale : 0.f;
           }
-          pd[e] = pdv;
-          ds[e] = ok ? pr * (dp - delta) * p.scale : 0.f;
+          st_swz128_u32(sP, r_loc[e], 8 * jj + 2 * q4, Elem<kBF16>::pack(pd[0], pd[1]));
+          st_swz128_u32(sDS, r_loc[e], 8 * jj + 2 * q4, Elem<kBF16>::pack(ds[0], ds[1]));
         }
-        uint4 u;
-        u.x = Elem<kBF16>::pack(pd[0], pd[1]); u.y = Elem<kBF16>::pack(pd[2], pd[3]);
-        u.z = Elem<kBF16>::pack(pd[4], pd[5]); u.w = Elem<kBF16>::pack(pd[6], pd[7]);
-        st_swz128(sP, row_t, col0, u);
-        u.x = Elem<kBF16>::pack(ds[0], ds[1]); u.y = Elem<kBF16>::pack(ds[2], ds[3]);
-        u.z = Elem<kBF16>::pack(ds[4], ds[5]); u.w = Elem<kBF16>::pack(ds[6], ds[7]);
-        st_swz128(sDS, row_t, col0, u);
-      }
-    }
-    if (pair) {   // exact zeros in the other head's key columns of this row
-      const int zc = ((1 - half) * 2 + chalf) * 32;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        st_swz128(sP, row_t, zc + g * 8, make_uint4(0, 0, 0, 0));
-        st_swz128(sDS, row_t, zc + g * 8, make_uint4(0, 0, 0, 0));
       }
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      // dV += Pd^T dO ; dK += dS^T Q : A = [queries x keys] read MN-major (M = keys),
-      // B = [queries x d] read MN-major (N = d); contraction over the q_pad query rows.
-      const uint32_t idesc_t = umma_idesc(fmt, 1, 1, ATT_BM, ATT_D);
-      const int nq16 = q_pad >> 4;
-      for (int kk = 0; kk < nq16; ++kk) {
-        umma_ss(tdV, umma_smem_desc(smem_u32(sP) + kk * 2048, ATT_TILE, 1024),
-                umma_smem_desc(smem_u32(sdO) + kk * 2048, 8192, 1024), idesc_t, (i | kk) != 0);
-      }
-      for (int kk = 0; kk < nq16; ++kk) {
-        umma_ss(tdK, umma_smem_desc(smem_u32(sDS) + kk * 2048, ATT_TILE, 1024),
-                umma_smem_desc(smem_u32(sQ) + kk * 2048, 8192, 1024), idesc_t, (i | kk) != 0);
-      }
-      // dQ = dS K : A K-major over keys, B = K_j [keys x d] MN-major
-      const uint32_t idesc_q = umma_idesc(fmt, 0, 1, ATT_BM, ATT_D);
-      const int nk16 = n_pad >> 4;
-      for (int kk = 0; kk < nk16; ++kk) {
-        umma_ss(tdQ, umma_smem_desc(smem_u32(sDS) + (kk >> 2) * ATT_TILE + (kk & 3) * 32, 16, 1024),
-                umma_smem_desc(smem_u32(sK) + kk * 2048, 8192, 1024), idesc_q, kk != 0);
-      }
-      umma_commit(bar_mma);
-    }
-    mbar_wait(bar_mma, ph_mma);
-    ph_mma ^= 1;
-    tc_fence_after();
-    // dQ_i out (rows = queries); each thread of the pair writes one 32-column half
-    {
-      const int cc = chalf;
-      uint32_t r[32];
-      tmem_ld32(tdQ + lane_off + cc * 32, r);
-      tmem_ld_wait();
-      if (p.dbias)   // query-bias gradient: this key block's share of colsum(dQ) for `head`
-        warp_colsum32_atomic(r, q_ok, p.dbias + head * ATT_D + cc * 32, tid & 31);
-      if (q_ok) {
-        if (nkv == 1) {
-          T16* out = reinterpret_cast<T16*>(p.dqkv) + static_cast<size_t>(seq0 + qrow) * (3 * p.H) +
-                     head * ATT_D + cc * 32;
+
+    float dq[32];
+    wgmma_fence();
+    // dV += Pd^T dO ; dK += dS^T Q : A = [queries x keys] read MN-major (M = keys of this
+    // warpgroup = slab wg), B = [queries x d] read MN-major (N = d); contraction over 128 queries.
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4 u;
-            u.x = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 0]), __uint_as_float(r[g * 8 + 1]));
-            u.y = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 2]), __uint_as_float(r[g * 8 + 3]));
-            u.z = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 4]), __uint_as_float(r[g * 8 + 5]));
-            u.w = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 6]), __uint_as_float(r[g * 8 + 7]));
-            *reinterpret_cast<uint4*>(out + g * 8) = u;
-          }
-        } else {
-          float* acc = dq_accum + static_cast<size_t>(seq0 + qrow) * p.H + head * ATT_D + cc * 32;
+    for (int kk = 0; kk < ATT_BM / 16; ++kk)
+      Wgmma<64, kBF16, 1, 1>::ss(dv, gmma_desc(uP + wg * ATT_TILE + kk * 2048, ATT_TILE, 1024),
+                                 gmma_desc(udO + kk * 2048, 8192, 1024), (i | kk) != 0);
 #pragma unroll
-          for (int e = 0; e < 32; ++e) atomicAdd(acc + e, __uint_as_float(r[e]));
+    for (int kk = 0; kk < ATT_BM / 16; ++kk)
+      Wgmma<64, kBF16, 1, 1>::ss(dk, gmma_desc(uDS + wg * ATT_TILE + kk * 2048, ATT_TILE, 1024),
+                                 gmma_desc(uQ + kk * 2048, 8192, 1024), (i | kk) != 0);
+    // dQ = dS K : A K-major over keys (rows = this warpgroup's queries), B = K_j [keys x d] MN-major
+#pragma unroll
+    for (int kk = 0; kk < ATT_BN / 16; ++kk)
+      Wgmma<64, kBF16, 0, 1>::ss(dq, gmma_desc(uDS + (kk >> 2) * ATT_TILE + wg * (64 * 128) + (kk & 3) * 32, 16, 1024),
+                                 gmma_desc(uK + kk * 2048, 8192, 1024), kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (p.dbias)   // query-bias gradient: this key block's share of colsum(dQ) for `head`
+      frag_colsum64_atomic(dq, q_ok[0], q_ok[1], p.dbias + head * ATT_D, lane);
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      if (!q_ok[e]) continue;
+      if (nkv == 1) {
+        store_frag_row<kBF16>(reinterpret_cast<T16*>(p.dqkv) + static_cast<size_t>(seq0 + qrow[e]) * (3 * p.H) +
+                                  head * ATT_D, dq, e, q4, 1.f);
+      } else {
+        float* acc = dq_accum + static_cast<size_t>(seq0 + qrow[e]) * p.H + head * ATT_D;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          atomicAdd(acc + 8 * jj + 2 * q4, dq[4 * jj + 2 * e]);
+          atomicAdd(acc + 8 * jj + 2 * q4 + 1, dq[4 * jj + 2 * e + 1]);
         }
       }
     }
-    if (i + 1 < nq) {  // next iteration overwrites S / dP / dQ (TMEM) and sQ / sdO / sP / sDS
-      tc_fence_before();
-      __syncthreads();
-      tc_fence_after();
-    }
+    if (i + 1 < nq) __syncthreads();   // next iteration overwrites sQ / sdO / sP / sDS
   }
 
   // dK_j, dV_j out (rows = keys)
-  {
-    const int key = pair ? (row_t & 63) : j * ATT_BN + row_t;
-    const bool k_ok = key < S;
-    T16* outk = reinterpret_cast<T16*>(p.dqkv) + static_cast<size_t>(seq0 + key) * (3 * p.H) +
-                p.H + head * ATT_D;
-    T16* outv = outk + p.H;
+  int key[2];
+  bool k_ok[2];
 #pragma unroll
-    for (int which = 0; which < 2; ++which) {
-      {
-        const int cc = chalf;
-        uint32_t r[32];
-        tmem_ld32((which ? tdV : tdK) + lane_off + cc * 32, r);
-        tmem_ld_wait();
-        if (p.dbias)   // key / value bias gradients
-          warp_colsum32_atomic(r, k_ok, p.dbias + (which ? 2 : 1) * p.H + head * ATT_D + cc * 32, tid & 31);
-        if (k_ok) {
-          T16* out = (which ? outv : outk) + cc * 32;
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4 u;
-            u.x = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 0]), __uint_as_float(r[g * 8 + 1]));
-            u.y = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 2]), __uint_as_float(r[g * 8 + 3]));
-            u.z = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 4]), __uint_as_float(r[g * 8 + 5]));
-            u.w = Elem<kBF16>::pack(__uint_as_float(r[g * 8 + 6]), __uint_as_float(r[g * 8 + 7]));
-            *reinterpret_cast<uint4*>(out + g * 8) = u;
-          }
-        }
-      }
-    }
+  for (int e = 0; e < 2; ++e) {
+    key[e] = pair ? (r_loc[e] & 63) : j * ATT_BN + r_loc[e];
+    k_ok[e] = key[e] < S;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, kSingle ? 256 : 512);
+  if (p.dbias) {   // key / value bias gradients
+    frag_colsum64_atomic(dk, k_ok[0], k_ok[1], p.dbias + p.H + head * ATT_D, lane);
+    frag_colsum64_atomic(dv, k_ok[0], k_ok[1], p.dbias + 2 * p.H + head * ATT_D, lane);
+  }
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    if (!k_ok[e]) continue;
+    T16* outk = reinterpret_cast<T16*>(p.dqkv) + static_cast<size_t>(seq0 + key[e]) * (3 * p.H) + p.H +
+                head * ATT_D;
+    store_frag_row<kBF16>(outk, dk, e, q4, 1.f);
+    store_frag_row<kBF16>(outk + p.H, dv, e, q4, 1.f);
   }
 }
 
@@ -650,7 +568,6 @@ __global__ void attn_dq_convert_kernel(const float* __restrict__ acc, void* dqkv
 }
 
 constexpr int ATT_BWD_SMEM = 8 * ATT_TILE + 64 + 1024;
-constexpr int ATT_BWD_SMEM_SINGLE = 7 * ATT_TILE + 64;
 
 }  // namespace ub
 
@@ -694,23 +611,15 @@ extern "C" int ub200_attn_fwd(const ub200_attn_args* args, ub200_stream_t stream
   p.rng_dev = reinterpret_cast<const unsigned long long*>(a.rng_offset_dev);
 
   dim3 grid((a.max_seqlen + ATT_BM - 1) / ATT_BM, a.num_heads, a.batch);
-  const bool single = a.max_seqlen <= ATT_BN;
   const bool bf = a.dtype == UB200_BF16;
   void (*kern)(const CUtensorMap, const CUtensorMap, const AttnParams) =
-      single ? (bf ? attn_fwd_kernel<true, true> : attn_fwd_kernel<false, true>)
-             : (bf ? attn_fwd_kernel<true, false> : attn_fwd_kernel<false, false>);
-  const int smem_bytes = single ? ATT_FWD_SMEM_SINGLE : ATT_FWD_SMEM;
-  static unsigned long long configured[4] = {0, 0, 0, 0};   // one bit per device
-  const int ci = (single ? 2 : 0) + (bf ? 1 : 0);
-  if (first_use_on_device(configured[ci])) {
-    UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    if (single)   // 4 CTAs x 49 KB per SM: ask for the full shared-memory carve-out
-      UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                         cudaSharedmemCarveoutMaxShared));
-  }
+      bf ? attn_fwd_kernel<true> : attn_fwd_kernel<false>;
+  static unsigned long long configured[2] = {0, 0};   // one bit per device
+  if (first_use_on_device(configured[bf ? 1 : 0]))
+    UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_FWD_SMEM));
   {
     ProfScope ps(stream);
-    UB_CHECK_CUDA(launch_pdl(kern, grid, dim3(128), smem_bytes, stream, 1, tm, tm64, p));
+    UB_CHECK_CUDA(launch_pdl(kern, grid, dim3(ATT_THREADS), ATT_FWD_SMEM, stream, 1, tm, tm64, p));
   }
   UB_CHECK_CUDA(cudaGetLastError());
   return 0;
@@ -769,24 +678,15 @@ extern "C" int ub200_attn_bwd(const ub200_attn_args* args, ub200_stream_t stream
     UB_CHECK_CUDA(cudaMemsetAsync(acc, 0, static_cast<size_t>(a.total_tokens) * a.hidden * 4, stream));
 
   dim3 grid((a.max_seqlen + ATT_BN - 1) / ATT_BN, a.num_heads, a.batch);
-  const bool single = !multi;
   const int di = a.dtype == UB200_BF16 ? 1 : 0;
   void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnParams,
-               float*) =
-      single ? (di ? attn_bwd_kernel<true, true> : attn_bwd_kernel<false, true>)
-             : (di ? attn_bwd_kernel<true, false> : attn_bwd_kernel<false, false>);
-  const int smem_bytes = single ? ATT_BWD_SMEM_SINGLE : ATT_BWD_SMEM;
-  static unsigned long long configured[4] = {0, 0, 0, 0};   // one bit per device
-  const int ci = (single ? 2 : 0) + di;
-  if (first_use_on_device(configured[ci])) {
-    UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    if (single)
-      UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                         cudaSharedmemCarveoutMaxShared));
-  }
+               float*) = di ? attn_bwd_kernel<true> : attn_bwd_kernel<false>;
+  static unsigned long long configured[2] = {0, 0};   // one bit per device
+  if (first_use_on_device(configured[di]))
+    UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_BWD_SMEM));
   {
     ProfScope ps(stream);
-    UB_CHECK_CUDA(launch_pdl(kern, grid, dim3(256), smem_bytes, stream, 1, tmQ, tmD, tmQ64, tmD64, p, acc));
+    UB_CHECK_CUDA(launch_pdl(kern, grid, dim3(ATT_THREADS), ATT_BWD_SMEM, stream, 1, tmQ, tmD, tmQ64, tmD64, p, acc));
   }
   UB_CHECK_CUDA(cudaGetLastError());
   if (multi) {

@@ -1,4 +1,4 @@
-// C entry point of the tcgen05 GEMM core: argument checks, tile / cluster selection, TMA
+// C entry point of the wgmma GEMM core: argument checks, tile / cluster selection, TMA
 // descriptors.  Device code lives in gemm_impl.cuh (instantiated in gemm_bf16.cu / gemm_f16.cu).
 #include <stdlib.h>
 
@@ -17,11 +17,10 @@ int launch_gemm_ln(int dtype, const GemmParams& p, const void* gamma, const void
                    long long ldy, const CUtensorMap& tmA, const CUtensorMap& tmB, cudaStream_t stream);
 
 // Pick (N tile, CTAs per tile) minimising  waves x k-blocks x cycles-per-k-block + exposed tail.
-// Cycles per k-block are MEASURED on B200 (K = 12288 sweep, mainloop only): they are far from
-// proportional to the tile width — 1-SM: ~421 + 1.27*BN (583 @128, 745 @256); 2-SM pair:
-// ~552 + 0.59*BN per 256-row pair tile (627 @128, 702 @256) — so fewer, wider tiles win until
-// wave quantisation bites.  The epilogue of the last tile (~25 cycles per column of width) and
-// a fixed launch / prologue cost are exposed once.
+// The cost model is a heuristic: a fixed per-k-block cost plus a part proportional to the tile
+// width (cheaper per column for a 2-CTA cluster, whose B tile is fetched once per pair), so fewer,
+// wider tiles win until wave quantisation bites.  The epilogue of the last tile and a fixed
+// launch / prologue cost are exposed once.  Its constants have not been re-fitted on H100.
 static void pick_config(int M, int N, int K, int sms, int* bn_out, int* cluster_out) {
   const int tiles_m = (M + BM - 1) / BM;
   const int num_kb = (K + BK - 1) / BK;
@@ -137,7 +136,7 @@ extern "C" int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream_) {
   else
     rc = make_tma_2d(&tmA, a.a, a.dtype, a.K, a.M, a.lda, BK, 64);
   if (rc) return rc;
-  if (a.b_major == 0)  // in 2-SM mode each CTA stages half of the B rows
+  if (a.b_major == 0)  // in 2-CTA clusters each CTA loads (and multicasts) half of the B rows
     rc = make_tma_2d(&tmB, a.b, a.dtype, n_valid, a.K, a.ldb, bn / cluster, BK);
   else
     rc = make_tma_2d(&tmB, a.b, a.dtype, a.K, n_valid, a.ldb, BK, 64);
@@ -205,9 +204,8 @@ extern "C" int ub200_gemm_grouped(const ub200_gemm_args* args, int32_t count, ub
     UB_CHECK_ARG(a.M > 0 && a.N > 0 && a.K > 0 && a.N % 8 == 0 && a.ldo % 8 == 0,
                  "gemm_grouped[%d]: bad shape", i);
   }
-  // N tile shared by the group: fewest (rounds over the SMs) x (measured cycles per k-block of a
-  // 128 x bn tile, see pick_config) — 4 base-layer wgrads: 432 tiles of 128 = 3 rounds x 583,
-  // 288 tiles of 192 = 2 rounds x 665, 216 tiles of 256 = 2 rounds x 745.
+  // N tile shared by the group: fewest (rounds over the SMs) x (cost per k-block of a 128 x bn tile,
+  // the same unmeasured heuristic as pick_config's: wider tiles cost less per column).
   const int sms = num_sms();
   int bn = args[0].tile_n;
   if (bn == 0) {

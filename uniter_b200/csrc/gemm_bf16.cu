@@ -1,4 +1,4 @@
-// bf16 instantiations of the tcgen05 GEMM core (split from fp16 for build parallelism).
+// bf16 instantiations of the wgmma GEMM core (split from fp16 for build parallelism).
 #include "gemm_impl.cuh"
 namespace ub {
 int gemm_dispatch_bf16(int bn, int cluster, int a_major, int b_major, const GemmParams& p,

@@ -1,4 +1,4 @@
-// fp16 instantiations of the tcgen05 GEMM core (split from bf16 for build parallelism).
+// fp16 instantiations of the wgmma GEMM core (split from bf16 for build parallelism).
 #include "gemm_impl.cuh"
 namespace ub {
 int gemm_dispatch_f16(int bn, int cluster, int a_major, int b_major, const GemmParams& p,

@@ -1,68 +1,49 @@
-// tcgen05 / TMA GEMM core for sm_100a.
+// wgmma / TMA GEMM core for sm_90a.
 //
-//   D[M,N] = epilogue( sum_k A[m,k] * B[n,k] ),  16-bit operands, fp32 accumulation in TMEM.
+//   D[M,N] = epilogue( sum_k A[m,k] * B[n,k] ),  16-bit operands, fp32 accumulation in registers.
 //
-// One persistent CTA per SM, 12 or 16 warps with fixed roles:
-//   warp 0      TMA producer   — one lane streams 128xBK A tiles and BNxBK B tiles into a
-//                                128B-swizzled smem ring (mbarrier full/empty pairs)
-//   warp 1      MMA issuer     — one lane issues tcgen05.mma (M=128, N=BN, K=16) x4 per stage,
-//                                tcgen05.commit releases smem slots and publishes accumulators
-//   warp 2      TMEM allocator — 2 x BN fp32 columns (double-buffered accumulator)
-//   warps 4-..  epilogue       — 2 (3 for BN = 192) warps per TMEM lane quarter (each takes a share of the BN
-//                                columns): tcgen05.ld 32 lanes x 32 columns, bias / dropout /
-//                                residual / GELU / dGELU / accumulate / column-sum, 16-byte stores
-// The mainloop of tile i+1 overlaps the epilogue of tile i through the two TMEM buffers.
+// One persistent CTA per SM, three warpgroups with fixed roles:
+//   warpgroup 0     TMA producer — one lane streams 128xBK A tiles and BNxBK B tiles into a
+//                   128B-swizzled smem ring (mbarrier full/empty pairs); the warpgroup gives
+//                   most of its registers to the consumers (setmaxnreg)
+//   warpgroups 1-2  consumers — each owns 64 rows of the 128 x BN tile: 4 x wgmma m64nBNk16 per
+//                   stage, a stage is released once the next stage's wgmma group is in flight;
+//                   then the epilogue from the accumulator registers: bias / dropout / residual /
+//                   GELU / dGELU / accumulate / column-sum, 16-byte stores
+// The producer runs ahead into the next tile while the consumers are in the epilogue.
 //
-// Two kernels share the epilogue:
-//   gemm_kernel      cta_group::1, tile 128 x BN per CTA.  Its mainloop is bound by shared-memory
-//                    bandwidth, not by the tensor pipe: per k-block TMA writes 16 KB + BN*128 B
-//                    and the SS-mode MMAs read the same amount again (96 KB at BN=256 = 750
-//                    cycles at 128 B/clk vs 512 MMA cycles) — measured 1000 cycles per k-block.
-//   gemm2sm_kernel   cta_group::2, tile 256 x BN per CTA PAIR (2-CTA cluster on one TPC).  Each
-//                    CTA stages its own 128 A rows and HALF of the B rows; one thread of the
-//                    leader CTA issues M=256 MMAs that read both CTAs' smem, so smem traffic per
-//                    CTA drops to 64 KB per k-block (500 cycles) for the same FLOPs.  TMA loads
-//                    of both CTAs complete on the leader's full barrier; tcgen05.commit
-//                    multicasts slot-free / accumulator-ready arrivals to both CTAs; the peer's
-//                    epilogue warps arrive remotely on the leader's tmem-empty barrier.
+// kCluster = 2: a cluster of two CTAs on neighbouring 128-row tiles of the same BN columns.  Each
+// CTA loads its own A tile and HALF of the B tile, multicast into both CTAs, so every B tile is
+// fetched from L2 once per pair.  A slot is refilled only after the consumers of BOTH CTAs have
+// released it (they arrive on the empty barrier of both).
 //
 // Operands may be K-major (contraction dim contiguous; nn.Linear forward) or MN-major
 // (contraction dim strided; dgrad reads the weight un-transposed, wgrad reads both activation
-// matrices un-transposed) — the UMMA descriptors encode the difference, no transposes are
+// matrices un-transposed) — the wgmma descriptors and transpose bits encode the difference, no transposes are
 // ever materialised.  Reference call sites replaced: model/layer.py:76-78,112,140,153 and
 // their autograd mirrors.
 #pragma once
 #include "common.h"
 #include "gemm_params.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace ub {
 
 constexpr int A_TILE_BYTES = BM * BK * 2;
-// Epilogue warps: a warp can only read the TMEM lane quarter (warp % 4), so more warps means
-// splitting the BN columns further.  ncu on the K = 768 GEMMs (3 tiles per CTA or one fully exposed
-// tile) showed the epilogue issue-bound with 2 warps per scheduler at 46 % issue utilisation; the
-// 192-wide tile (6 column blocks) is split 3 ways -> 12 epilogue warps, 3 per scheduler.  (256-wide
-// tiles stay at 2: their 4-stage ring leaves no shared memory for more transpose buffers.)
-constexpr int epi_split(int bn) { return bn == 192 ? 3 : 2; }
-constexpr int epi_warps(int bn) { return 4 * epi_split(bn); }
-constexpr int gemm_threads(int bn) { return 128 + 32 * epi_warps(bn); }   // 384 or 512
+constexpr int GEMM_THREADS = 384;       // producer warpgroup + 2 consumer warpgroups
+constexpr int EPI_WARPS = 8;            // consumer warps, 16 accumulator rows each
+constexpr int EPI_PITCH = 33;           // fp32 words per row of a warp's 16 x 32 transpose buffer
 
-template <int BN, int kCtas>
+template <int BN>
 struct GemmCfg {
-  static constexpr int B_TILE_BYTES = BN / kCtas * BK * 2;   // per CTA
+  static constexpr int B_TILE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
-  static constexpr int STAGES = (192 * 1024) / STAGE_BYTES > 8 ? 8 : (192 * 1024) / STAGE_BYTES;
-  // two accumulators of BN fp32 columns; allocations must be a power of two >= 32
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : ((2 * BN <= 256) ? 256 : 512);
+  static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
   static constexpr int BAR_BYTES = 256;
-  static constexpr int EPI_WARPS = epi_warps(BN);
-  static constexpr int THREADS = gemm_threads(BN);
-  // per epilogue warp: 32 x 33 fp32 transpose buffer (lane == row  ->  4 lanes per row)
-  static constexpr int EPI_STAGE_BYTES = EPI_WARPS * 32 * 33 * 4;
+  static constexpr int EPI_STAGE_BYTES = EPI_WARPS * 16 * EPI_PITCH * 4;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + EPI_STAGE_BYTES + 1024;  // + align slack
 };
-
 
 template <bool kBF16>
 __device__ __forceinline__ void load8(const void* base, long long idx, float (&f)[8]) {
@@ -93,35 +74,15 @@ __device__ __forceinline__ void store8(void* base, long long idx, const float (&
 }
 
 
-// Bring-up instrumentation, compiled only with -DUB200_BRINGUP (never in the shipped library):
-// epilogue bit 27 turns p.colsum into a per-CTA timeline buffer (clock64 stamps), bit 30 drops a
-// tile's epilogue, bit 29 drops its stores.
-#ifdef UB200_BRINGUP
-#define UB_TRACE(slot)                                                                      \
-  do {                                                                                      \
-    if (p.epilogue & (1 << 27))                                                             \
-      reinterpret_cast<long long*>(p.colsum)[blockIdx.x * 16 + (slot)] = clock64();         \
-  } while (0)
-#define UB_BRINGUP_HAS(E, bit) (E).has(bit)
-#else
-#define UB_TRACE(slot) do { } while (0)
-#define UB_BRINGUP_HAS(E, bit) false
-#endif
-
 // --------------------------------------------------------------------------------- epilogue
-// One epilogue warp: rows = TMEM lanes [32*quarter, +32) of the CTA's 128-row accumulator (this
-// thread owns global row `row`), columns = half `chalf` of the BN columns, in 32-column blocks.
-// `t_acc` already includes the lane offset.
+// One consumer warp: 16 accumulator rows [row0, row0 + 16) x BN columns from n0, in 32-column
+// blocks.  Accumulator register i of the wgmma fragment holds row (lane / 4) + 8 * ((i / 2) % 2),
+// column 8 * (i / 4) + 2 * (lane % 4) + i % 2.
 //
-// Measured (clock64 timeline, 128x256 tile): the TMEM loads take ~1.7k cycles per tile but the
-// first version of this function took ~12k — twice the K=768 mainloop — because ~230 mostly
-// dependent instructions per block (38 branches on runtime flags, loads used immediately)
-// ran with 2 warps per SM sub-partition and no ILP.  Hence:
 //   * EPI >= 0 is a compile-time epilogue mask (the combinations the encoder uses are
 //     instantiated; EPI < 0 falls back to the runtime mask in p.epilogue);
-//   * side inputs of a block (bias / residual / dGELU aux / accumulate) are requested before
-//     waiting for the TMEM load, and the TMEM load of block i+1 is in flight while block i is
-//     processed (two register buffers).
+//   * side inputs of a block (bias / residual / dGELU aux / accumulate) are requested before the
+//     block is staged.
 template <int EPI, bool kBF16>
 struct EpiMask {
   const int rt;
@@ -129,20 +90,25 @@ struct EpiMask {
   __device__ __forceinline__ bool has(int bit) const { return EPI >= 0 ? (EPI & bit) != 0 : (rt & bit) != 0; }
 };
 
-// tcgen05.ld delivers lane == row.  Storing (or loading side inputs) in that mapping makes every
-// warp-level LDG / STG touch 32 different rows = 32 line transactions, and the LSU backs up
-// (ncu: long-scoreboard stalls on the instruction that recycles a store's registers; ~12k cycles
-// per 128x256 tile, twice the K=768 mainloop).  Each 32x32 block therefore goes through a
-// per-warp smem transpose (pitch 33 words: conflict-free both ways) after which 4 lanes own
-// one row: every global access of the warp covers 8 rows x 64 contiguous bytes, side inputs
-// are requested before the TMEM wait, and the column sum needs 3 shuffle steps.
+// The fragment scatters a row over 4 lanes in 2-column pieces; storing (or loading side inputs)
+// in that mapping makes every warp-level access touch 8 rows in 8-byte pieces.  Each 16 x 32 block
+// therefore goes through a per-warp smem transpose (pitch 33 words) after which 4 lanes own one
+// row: every global access of the warp covers 8 rows x 64 contiguous bytes and the column sum
+// needs 3 shuffle steps.
+template <int BN>
+__device__ __forceinline__ void stage_block(const float (&acc)[BN / 2], int c, int lane, float* stage) {
+#pragma unroll
+  for (int t = 0; t < 16; ++t) {
+    const int r = (lane >> 2) + 8 * ((t >> 1) & 1);
+    const int cc = 8 * (t >> 2) + 2 * (lane & 3) + (t & 1);
+    stage[r * EPI_PITCH + cc] = acc[16 * c + t];
+  }
+}
+
 template <int EPI, int BN, bool kBF16>
-__device__ __forceinline__ void epilogue_warp(const GemmParams& p, uint32_t t_acc, int row0, int n0,
-                                              int chalf, int lane, const DropoutRng& rng,
-                                              float* stage, uint64_t* empty_bar_local,
-                                              uint32_t empty_bar_cluster, bool remote_arrive) {
+__device__ __forceinline__ void epilogue_warp(const GemmParams& p, const float (&acc)[BN / 2], int row0, int n0,
+                                              int lane, const DropoutRng& rng, float* stage) {
   using T16 = typename Elem<kBF16>::T;
-  constexpr int CHUNKS = BN / 32 / epi_split(BN);
   const EpiMask<EPI, kBF16> E(p.epilogue);
   const int sub_r = lane >> 2;        // row inside an 8-row group
   const int cg = (lane & 3) * 8;      // first of this lane's 8 columns inside the 32-column block
@@ -152,47 +118,30 @@ __device__ __forceinline__ void epilogue_warp(const GemmParams& p, uint32_t t_ac
                          : (E.has(UB200_EPI_DGELU) ? reinterpret_cast<const T16*>(p.aux)
                                                    : reinterpret_cast<const T16*>(p.out));
   const long long side_ld = E.has(UB200_EPI_RESIDUAL) ? p.ldr : (E.has(UB200_EPI_DGELU) ? p.ldaux : p.ldo);
-#pragma unroll 1
-  for (int cw = 0; cw < CHUNKS; ++cw) {
-    const int c = chalf * CHUNKS + cw;
-    uint32_t r[32];
-    tmem_ld32(t_acc + c * 32, r);
+#pragma unroll
+  for (int c = 0; c < BN / 32; ++c) {
     const int col0 = n0 + c * 32;
+    if (col0 >= p.N) break;           // warp-uniform
     const int col = col0 + cg;
     const bool col_ok = col < p.N;    // N % 8 == 0 is enforced on the host
-    // ---- side inputs in the coalesced mapping, requested while the TMEM load is in flight
     uint4 bias4 = make_uint4(0, 0, 0, 0);
-    uint4 side[4];
+    uint4 side[2];
 #pragma unroll
-    for (int it = 0; it < 4; ++it) side[it] = make_uint4(0, 0, 0, 0);
+    for (int it = 0; it < 2; ++it) side[it] = make_uint4(0, 0, 0, 0);
     if (col_ok) {
       if (E.has(UB200_EPI_BIAS))
         bias4 = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.bias) + col));
       if (side16) {
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
+        for (int it = 0; it < 2; ++it) {
           const int row = row0 + it * 8 + sub_r;
           if (row < p.M)
             side[it] = __ldg(reinterpret_cast<const uint4*>(side_base + static_cast<long long>(row) * side_ld + col));
         }
       }
     }
-    tmem_ld_wait();
-    if (cw == CHUNKS - 1) {
-      // all of this warp's TMEM reads for the tile are done: hand the buffer back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (remote_arrive) mbar_arrive_cluster(empty_bar_cluster);
-        else mbar_arrive(empty_bar_local);
-      }
-    }
-    if (col0 >= p.N) continue;        // warp-uniform
-    if (UB_BRINGUP_HAS(E, 1 << 30)) continue;   // bring-up only: drop the tile
-
     __syncwarp();                     // previous block's readers are done with `stage`
-#pragma unroll
-    for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = __uint_as_float(r[j]);
+    stage_block<BN>(acc, c, lane, stage);
     __syncwarp();
 
     float bias8[8];
@@ -202,12 +151,12 @@ __device__ __forceinline__ void epilogue_warp(const GemmParams& p, uint32_t t_ac
     for (int i = 0; i < 8; ++i) csum[i] = 0.f;
 
 #pragma unroll
-    for (int it = 0; it < 4; ++it) {
+    for (int it = 0; it < 2; ++it) {
       const int rr = it * 8 + sub_r;
       const int row = row0 + rr;
       float v[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = stage[rr * 33 + cg + i] + bias8[i];
+      for (int i = 0; i < 8; ++i) v[i] = stage[rr * EPI_PITCH + cg + i] + bias8[i];
       if (!(col_ok && row < p.M)) continue;
       if (E.has(UB200_EPI_DROPOUT)) {
         const uint64_t e = static_cast<uint64_t>(row) * static_cast<uint64_t>(p.N) + col;
@@ -269,7 +218,7 @@ __device__ __forceinline__ void epilogue_warp(const GemmParams& p, uint32_t t_ac
 #pragma unroll
           for (int i = 0; i < 8; ++i) v[i] += t[i];
         }
-        if (!UB_BRINGUP_HAS(E, 1 << 29)) store8<kBF16>(p.out, static_cast<long long>(row) * p.ldo + col, v);
+        store8<kBF16>(p.out, static_cast<long long>(row) * p.ldo + col, v);
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i) csum[i] += v[i];
@@ -293,7 +242,6 @@ __device__ __forceinline__ void epilogue_warp(const GemmParams& p, uint32_t t_ac
 }
 
 
-
 __device__ __forceinline__ DropoutRng make_rng(const GemmParams& p) {
   DropoutRng rng;
   rng.k0 = p.seed_lo; rng.k1 = p.seed_hi; rng.s0 = p.stream_lo; rng.s1 = p.stream_hi;
@@ -302,12 +250,100 @@ __device__ __forceinline__ DropoutRng make_rng(const GemmParams& p) {
   return rng;
 }
 
-// =================================================================================== 1-SM kernel
-template <int BN, bool A_MN, bool B_MN, bool kBF16, int EPI>
-__global__ void __launch_bounds__(gemm_threads(BN), 1)
+__device__ __forceinline__ void setmaxnreg_producer() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+}
+__device__ __forceinline__ void setmaxnreg_consumer() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+}
+
+// ------------------------------------------------------------------------------ pipeline halves
+// Producer lane: k-blocks [kb0, kb1) of the 128 x BN tile at (m0, n0) into the ring.  With
+// kCluster = 2 this CTA (cluster rank `rank`) loads half of the B tile and multicasts it.
+template <int BN, bool A_MN, bool B_MN, int kCluster>
+__device__ __forceinline__ void produce_tile(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                             const CUtensorMap* tmA, const CUtensorMap* tmB, int m0, int n0,
+                                             int kb0, int kb1, int& stage, uint32_t& phase, uint32_t rank) {
+  using Cfg = GemmCfg<BN>;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&empty_bar[stage], phase ^ 1);
+    uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
+    uint8_t* sB = sA + A_TILE_BYTES;
+    mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);   // own A + the whole B tile
+    if (!A_MN) {
+      tma_load_2d(sA, tmA, &full_bar[stage], kb * BK, m0);
+    } else {
+#pragma unroll
+      for (int j = 0; j < BM / 64; ++j)
+        tma_load_2d(sA + j * (64 * BK * 2), tmA, &full_bar[stage], m0 + j * 64, kb * BK);
+    }
+    if (kCluster == 1) {
+      if (!B_MN) {
+        tma_load_2d(sB, tmB, &full_bar[stage], kb * BK, n0);
+      } else {
+#pragma unroll
+        for (int j = 0; j < BN / 64; ++j)
+          tma_load_2d(sB + j * (64 * BK * 2), tmB, &full_bar[stage], n0 + j * 64, kb * BK);
+      }
+    } else {
+      constexpr int BH = BN / 2;
+      if (!B_MN) {
+        tma_load_2d_mc(sB + rank * (BH * BK * 2), tmB, &full_bar[stage], kb * BK, n0 + rank * BH, 3);
+      } else {
+#pragma unroll
+        for (int j = 0; j < BH / 64; ++j) {
+          const int jj = rank * (BH / 64) + j;
+          tma_load_2d_mc(sB + jj * (64 * BK * 2), tmB, &full_bar[stage], n0 + jj * 64, kb * BK, 3);
+        }
+      }
+    }
+    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+  }
+}
+
+// Consumer warpgroup `wg` (rows [64 wg, 64 wg + 64) of the tile): acc = A B^T over nkb k-blocks.
+// K-major operands advance 16 elements = 32 B inside the swizzle row per k16 step; MN-major ones
+// advance 16 K-rows = 2048 B, their 64-wide M/N groups are one 8 KB box apart.
+template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster>
+__device__ __forceinline__ void consume_tile(float (&acc)[BN / 2], uint8_t* smem, uint64_t* full_bar,
+                                             uint64_t* empty_bar, int nkb, int wg, int& stage,
+                                             uint32_t& phase, uint32_t peer) {
+  using Cfg = GemmCfg<BN>;
+  constexpr uint32_t A_KSTEP = A_MN ? 2048 : 32, A_LBO = A_MN ? 8192 : 16;
+  constexpr uint32_t B_KSTEP = B_MN ? 2048 : 32, B_LBO = B_MN ? 8192 : 16;
+  const bool releaser = (threadIdx.x & 127) == 0;
+  int prev = -1;
+  for (int kb = 0; kb < nkb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES) + wg * (64 * 128);
+    const uint32_t sB = smem_u32(smem + stage * Cfg::STAGE_BYTES) + A_TILE_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k)
+      Wgmma<BN, kBF16, A_MN, B_MN>::ss(acc, gmma_desc(sA + k * A_KSTEP, A_LBO, 1024),
+                                       gmma_desc(sB + k * B_KSTEP, B_LBO, 1024), (kb | k) != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();                   // the previous stage's wgmma group has retired
+    if (prev >= 0 && releaser) {
+      mbar_arrive(&empty_bar[prev]);
+      if (kCluster == 2) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[prev]), peer));
+    }
+    prev = stage;
+    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  if (releaser) {
+    mbar_arrive(&empty_bar[prev]);
+    if (kCluster == 2) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[prev]), peer));
+  }
+}
+
+// =================================================================================== GEMM kernel
+template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster, int EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const GemmParams p) {
-  using Cfg = GemmCfg<BN, 1>;
+  using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.  The offset is computed in the shared window
   // and applied by pointer arithmetic on the __shared__ array so that the compiler keeps the
@@ -315,160 +351,80 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::STAGES;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const uint32_t rank = kCluster == 2 ? cluster_ctarank() : 0u;
   const int num_kb = (p.K + BK - 1) / BK;
-  const int num_tiles = p.tiles_m * p.tiles_n;
+  const int num_tiles = p.tiles_n * (kCluster == 2 ? (p.tiles_m + 1) / 2 : p.tiles_m);
   // work unit = (tile, k-slice): unit % num_tiles is the tile, unit / num_tiles the slice of
-  // kb_per_split k-blocks (ksplit == 1: one slice covering all of K)
+  // kb_per_split k-blocks (ksplit == 1: one slice covering all of K).  A cluster pair shares one
+  // unit sequence; its tile is 256 rows high.
   const int num_units = num_tiles * p.ksplit;
-  if (threadIdx.x == 0) UB_TRACE(0);
+  const int unit0 = kCluster == 2 ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
+  const int unit_step = kCluster == 2 ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], Cfg::EPI_WARPS);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[s], 2 * kCluster);   // one arrive per consumer warpgroup (of both CTAs)
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
   pdl_launch_dependents();   // dependents may start their own prologue
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
+  if (kCluster == 2) cluster_sync_all();   // both CTAs' barriers exist before any multicast / remote arrive
   pdl_wait();                // the producing kernel has completed; its outputs are visible
-  if (threadIdx.x == 0) UB_TRACE(1);
 
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_producer();
     // ===================================================================== TMA producer
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+      for (int unit = unit0; unit < num_units; unit += unit_step) {
         const int tile = unit % num_tiles;
         const int kb0 = (unit / num_tiles) * p.kb_per_split;
         const int kb1 = min(num_kb, kb0 + p.kb_per_split);
-        const int m0 = (tile / p.tiles_n) * BM;
+        const int m0 = (tile / p.tiles_n) * (kCluster * BM) + static_cast<int>(rank) * BM;
         const int n0 = (tile % p.tiles_n) * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sB = sA + A_TILE_BYTES;
-          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          if (!A_MN) {
-            tma_load_2d(sA, &tmA, &full_bar[stage], kb * BK, m0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)
-              tma_load_2d(sA + j * (64 * BK * 2), &tmA, &full_bar[stage], m0 + j * 64, kb * BK);
-          }
-          if (!B_MN) {
-            tma_load_2d(sB, &tmB, &full_bar[stage], kb * BK, n0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
-              tma_load_2d(sB + j * (64 * BK * 2), &tmB, &full_bar[stage], n0 + j * 64, kb * BK);
-          }
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-          if (kb == kb0 && unit == static_cast<int>(blockIdx.x)) UB_TRACE(2);
-        }
-      }
-      UB_TRACE(3);
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(kBF16 ? 1 : 0, A_MN ? 1 : 0, B_MN ? 1 : 0, BM, BN);
-      // K-major: advance 16 elements = 32 B inside the swizzle row; 8-row groups 1024 B apart.
-      // MN-major: advance 16 K-rows = 2048 B; 64-wide M/N groups one 8 KB box apart.
-      constexpr uint32_t A_KSTEP = A_MN ? 2048 : 32, A_LBO = A_MN ? 8192 : 16;
-      constexpr uint32_t B_KSTEP = B_MN ? 2048 : 32, B_LBO = B_MN ? 8192 : 16;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
-        const int kb0 = (unit / num_tiles) * p.kb_per_split;
-        const int kb1 = min(num_kb, kb0 + p.kb_per_split);
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BN);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (kb == kb0 && unit == static_cast<int>(blockIdx.x)) UB_TRACE(4);
-          const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sB = sA + A_TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = umma_smem_desc(sA + k * A_KSTEP, A_LBO, 1024);
-            const uint64_t db = umma_smem_desc(sB + k * B_KSTEP, B_LBO, 1024);
-            umma_ss(d_tmem, da, db, idesc, ((kb - kb0) | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // smem slot free once these MMAs retire
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full_bar[acc]);  // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        UB_TRACE(5);   // last value = all MMAs of the last tile issued
+        produce_tile<BN, A_MN, B_MN, kCluster>(smem, full_bar, empty_bar, &tmA, &tmB, m0, n0, kb0, kb1,
+                                               stage, phase, rank);
       }
     }
-  } else if (warp >= 4) {
-    // ===================================================================== epilogue (8 warps)
-    const int quarter = warp & 3;         // TMEM lanes [32*quarter, 32*quarter+32)
-    const int chalf = (warp - 4) >> 2;    // which 1/epi_split(BN) of the BN columns this warp handles
+  } else {
+    setmaxnreg_consumer();
+    // ===================================================================== consumers + epilogue
+    const int cw = warp - 4;              // consumer warp 0..7
+    const int wg = cw >> 2;
     const DropoutRng rng = make_rng(p);
     float* epi_stage = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES) +
-                       (warp - 4) * (32 * 33);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+                       cw * (16 * EPI_PITCH);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int unit = unit0; unit < num_units; unit += unit_step) {
       const int tile = unit % num_tiles;
-      const int m0 = (tile / p.tiles_n) * BM;
+      const int kb0 = (unit / num_tiles) * p.kb_per_split;
+      const int kb1 = min(num_kb, kb0 + p.kb_per_split);
+      const int m0 = (tile / p.tiles_n) * (kCluster * BM) + static_cast<int>(rank) * BM;
       const int n0 = (tile % p.tiles_n) * BN;
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      if (warp == 4 && lane == 0) UB_TRACE(unit == static_cast<int>(blockIdx.x) ? 6 : 8);
-      const uint32_t t_acc = tmem_base + static_cast<uint32_t>(acc * BN) +
-                             (static_cast<uint32_t>(quarter * 32) << 16);
-      epilogue_warp<EPI, BN, kBF16>(p, t_acc, m0 + quarter * 32, n0, chalf, lane, rng, epi_stage,
-                                    &tmem_empty_bar[acc], 0u, false);
-      if (warp == 4 && lane == 0) UB_TRACE(unit == static_cast<int>(blockIdx.x) ? 7 : 9);
-      if (warp == 3 + Cfg::EPI_WARPS && lane == 0) UB_TRACE(10);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      consume_tile<BN, A_MN, B_MN, kBF16, kCluster>(acc, smem, full_bar, empty_bar, kb1 - kb0, wg, stage,
+                                                    phase, rank ^ 1u);
+      epilogue_warp<EPI, BN, kBF16>(p, acc, m0 + 16 * cw, n0, lane, rng, epi_stage);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) UB_TRACE(11);
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
+  if (kCluster == 2) cluster_sync_all();   // nobody exits while the peer may still signal it
 }
 
 // =================================================================================== grouped wgrad
 // The four weight-gradient GEMMs of a layer (dW2 = dY2^T f, dW1 = dPre^T a, dWo = dY1^T ctx,
 // dWqkv = dQKV^T x; all contract over K = T tokens, both operands MN-major) as ONE persistent
-// launch: 432 tiles of 128x128 on 148 SMs (2.9 balanced rounds) instead of four launches of
-// 144 / 144 / 36 / 108 tiles, each with its own prologue and exposed epilogue tail.
+// launch instead of four, each with its own prologue and exposed epilogue tail.
 struct TmPack {
   CUtensorMap a[GEMM_MAX_GROUP];
   CUtensorMap b[GEMM_MAX_GROUP];
@@ -483,47 +439,33 @@ __device__ __forceinline__ int group_of_tile(const GroupedParams& g, int tile) {
 }
 
 template <int BN, bool kBF16, int EPI>
-__global__ void __launch_bounds__(gemm_threads(BN), 1)
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
-  using Cfg = GemmCfg<BN, 1>;
+  using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::STAGES;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_kb = (g.K + BK - 1) / BK;
   const int num_tiles = g.tile_start[g.nprob];
 
-  if (warp == 1 && lane == 0) {
+  if (warp == 0 && lane == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], Cfg::EPI_WARPS);
+      mbar_init(&empty_bar[s], 2);
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
   pdl_launch_dependents();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
 
-  if (warp == 0) {
-    // ===================================================================== TMA producer
-    if (lane == 0) {
+  if (warp < 4) {
+    setmaxnreg_producer();
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -531,63 +473,23 @@ gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
         const int lt = tile - g.tile_start[pi];
         const int m0 = (lt / g.tiles_n[pi]) * BM;
         const int n0 = (lt % g.tiles_n[pi]) * BN;
-        const CUtensorMap* ta = &tm.a[pi];
-        const CUtensorMap* tb = &tm.b[pi];
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sB = sA + A_TILE_BYTES;
-          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-#pragma unroll
-          for (int j = 0; j < BM / 64; ++j)
-            tma_load_2d(sA + j * (64 * BK * 2), ta, &full_bar[stage], m0 + j * 64, kb * BK);
-#pragma unroll
-          for (int j = 0; j < BN / 64; ++j)
-            tma_load_2d(sB + j * (64 * BK * 2), tb, &full_bar[stage], n0 + j * 64, kb * BK);
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
+        produce_tile<BN, true, true, 1>(smem, full_bar, empty_bar, &tm.a[pi], &tm.b[pi], m0, n0, 0, num_kb,
+                                        stage, phase, 0u);
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(kBF16 ? 1 : 0, 1, 1, BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sB = sA + A_TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = umma_smem_desc(sA + k * 2048, 8192, 1024);
-            const uint64_t db = umma_smem_desc(sB + k * 2048, 8192, 1024);
-            umma_ss(d_tmem, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================================================================== epilogue (8 warps)
-    const int quarter = warp & 3;
-    const int chalf = (warp - 4) >> 2;
+  } else {
+    setmaxnreg_consumer();
+    const int cw = warp - 4;
+    const int wg = cw >> 2;
     DropoutRng rng;
     rng.k0 = rng.k1 = rng.s0 = rng.s1 = 0; rng.thr16 = 0; rng.inv_keep = 1.f;
     float* epi_stage = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES) +
-                       (warp - 4) * (32 * 33);
-    int acc = 0;
-    uint32_t acc_phase = 0;
+                       cw * (16 * EPI_PITCH);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int pi = group_of_tile(g, tile);
       const int lt = tile - g.tile_start[pi];
@@ -596,187 +498,24 @@ gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
       GemmParams pp{};
       pp.M = g.M[pi]; pp.N = g.N[pi]; pp.K = g.K; pp.epilogue = g.epilogue;
       pp.out = g.out[pi]; pp.ldo = g.ldo[pi];
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_acc = tmem_base + static_cast<uint32_t>(acc * BN) +
-                             (static_cast<uint32_t>(quarter * 32) << 16);
-      epilogue_warp<EPI, BN, kBF16>(pp, t_acc, m0 + quarter * 32, n0, chalf, lane, rng, epi_stage,
-                                    &tmem_empty_bar[acc], 0u, false);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      consume_tile<BN, true, true, kBF16, 1>(acc, smem, full_bar, empty_bar, num_kb, wg, stage, phase, 0u);
+      epilogue_warp<EPI, BN, kBF16>(pp, acc, m0 + 16 * cw, n0, lane, rng, epi_stage);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-// =================================================================================== 2-SM kernel
-// CTA pair (cluster of 2): output tile 256 x BN.  rank 0 = leader (issues the MMAs).
-template <int BN, bool A_MN, bool B_MN, bool kBF16, int EPI>
-__global__ void __launch_bounds__(gemm_threads(BN), 1)
-gemm2sm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const GemmParams p) {
-  using Cfg = GemmCfg<BN, 2>;
-  constexpr int BH = BN / 2;  // B rows staged by each CTA
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::STAGES;   // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int num_kb = (p.K + BK - 1) / BK;
-  const int pair_id = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-  const int num_units = ((p.tiles_m + 1) / 2) * p.tiles_n;   // tiles_m counts 128-row tiles
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);    // leader's expect_tx arrive; bytes of BOTH CTAs complete it
-      mbar_init(&empty_bar[s], 1);   // leader's multicast tcgen05.commit
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tmem_full_bar[a], 1);
-      mbar_init(&tmem_empty_bar[a], 2 * Cfg::EPI_WARPS);  // epilogue warps of BOTH CTAs (leader's copy)
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) {
-    tmem_alloc_2sm(tmem_ptr_smem, Cfg::TMEM_COLS);
-    tmem_relinquish_2sm();
-  }
-  pdl_launch_dependents();
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();   // both CTAs' barriers are initialised before any remote arrive / TMA signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  pdl_wait();
-
-  if (warp == 0) {
-    // ===================================================================== TMA producer (both CTAs)
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int unit = pair_id; unit < num_units; unit += num_pairs) {
-        const int m0 = (unit / p.tiles_n) * (2 * BM) + static_cast<int>(rank) * BM;
-        const int n0 = (unit % p.tiles_n) * BN + static_cast<int>(rank) * BH;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sB = sA + A_TILE_BYTES;
-          // transaction bytes of both CTAs are counted on the LEADER's full barrier
-          const uint32_t bar = mapa_shared(smem_u32(&full_bar[stage]), 0);
-          if (leader) mbar_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-          if (!A_MN) {
-            tma_load_2d_2sm(sA, &tmA, bar, kb * BK, m0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BM / 64; ++j)
-              tma_load_2d_2sm(sA + j * (64 * BK * 2), &tmA, bar, m0 + j * 64, kb * BK);
-          }
-          if (!B_MN) {
-            tma_load_2d_2sm(sB, &tmB, bar, kb * BK, n0);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BH / 64; ++j)
-              tma_load_2d_2sm(sB + j * (64 * BK * 2), &tmB, bar, n0 + j * 64, kb * BK);
-          }
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (leader only)
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(kBF16 ? 1 : 0, A_MN ? 1 : 0, B_MN ? 1 : 0, 2 * BM, BN);
-      constexpr uint32_t A_KSTEP = A_MN ? 2048 : 32, A_LBO = A_MN ? 8192 : 16;
-      constexpr uint32_t B_KSTEP = B_MN ? 2048 : 32, B_LBO = B_MN ? 8192 : 16;
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int unit = pair_id; unit < num_units; unit += num_pairs) {
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sB = sA + A_TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = umma_smem_desc(sA + k * A_KSTEP, A_LBO, 1024);
-            const uint64_t db = umma_smem_desc(sB + k * B_KSTEP, B_LBO, 1024);
-            umma_ss_2sm(d_tmem, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit_2sm(&empty_bar[stage], 3);   // slot free in both CTAs
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm(&tmem_full_bar[acc], 3);   // accumulator ready in both CTAs
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================================================================== epilogue (both CTAs)
-    const int quarter = warp & 3;
-    const int chalf = (warp - 4) >> 2;
-    const DropoutRng rng = make_rng(p);
-    float* epi_stage = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES) +
-                       (warp - 4) * (32 * 33);
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int unit = pair_id; unit < num_units; unit += num_pairs) {
-      const int m0 = (unit / p.tiles_n) * (2 * BM) + static_cast<int>(rank) * BM;
-      const int n0 = (unit % p.tiles_n) * BN;
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_acc = tmem_base + static_cast<uint32_t>(acc * BN) +
-                             (static_cast<uint32_t>(quarter * 32) << 16);
-      const uint32_t leader_empty = mapa_shared(smem_u32(&tmem_empty_bar[acc]), 0);
-      epilogue_warp<EPI, BN, kBF16>(p, t_acc, m0 + quarter * 32, n0, chalf, lane, rng, epi_stage,
-                                    &tmem_empty_bar[acc], leader_empty, true);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();   // nobody exits (or frees TMEM) while the peer may still signal / read
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, Cfg::TMEM_COLS);
   }
 }
 
 template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster, int EPI>
 static int launch_gemm(const GemmParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, int grid,
                        cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, kCluster>;
-  void (*kern)(const CUtensorMap, const CUtensorMap, const GemmParams);
-  if (kCluster == 2) kern = gemm2sm_kernel<BN, A_MN, B_MN, kBF16, EPI>;
-  else kern = gemm_kernel<BN, A_MN, B_MN, kBF16, EPI>;
+  using Cfg = GemmCfg<BN>;
+  void (*kern)(const CUtensorMap, const CUtensorMap, const GemmParams) = gemm_kernel<BN, A_MN, B_MN, kBF16, kCluster, EPI>;
   static unsigned long long configured = 0;  // per instantiation, one bit per device
   if (first_use_on_device(configured))
     UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        Cfg::SMEM_BYTES));
   {
     ProfScope ps(stream);
-    UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, kCluster,
+    UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, kCluster,
                              tmA, tmB, p));
   }
   return 0;
@@ -833,7 +572,7 @@ int gemm_dispatch(int bn, int cluster, int a_major, int b_major, const GemmParam
 
 template <int BN, bool kBF16>
 int gemm_group_launch(const TmPack& tm, const GroupedParams& g, int grid, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, 1>;
+  using Cfg = GemmCfg<BN>;
   void (*kern)(const TmPack, const GroupedParams);
   if (g.epilogue == 0) kern = gemm_group_kernel<BN, kBF16, 0>;
   else if (g.epilogue == UB200_EPI_ACCUM) kern = gemm_group_kernel<BN, kBF16, UB200_EPI_ACCUM>;
@@ -843,7 +582,7 @@ int gemm_group_launch(const TmPack& tm, const GroupedParams& g, int grid, cudaSt
   if (first_use_on_device(configured[ci]))
     UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   ProfScope ps(stream);
-  UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, 1, tm, g));
+  UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, 1, tm, g));
   return 0;
 }
 

@@ -5,7 +5,7 @@
 //
 // One kernel replaces GEMM(+bias+dropout+residual) -> s to HBM -> ln_fwd_kernel (read s, write y):
 // the row statistics need the whole row of N = H columns, which is wider than one CTA's accumulator
-// (128 x 768 fp32 = 768 TMEM columns > 512), so the row is split over a CLUSTER of 4 CTAs along N
+// (128 x 768 fp32 = 384 accumulator registers per consumer thread), so the row is split over a CLUSTER of 4 CTAs along N
 // (H = 768: 4 x 192, H = 1024: 4 x 256) that exchange per-row (mean, M2) through distributed shared
 // memory:
 //
@@ -13,13 +13,13 @@
 //           v = acc + bias -> dropout -> + residual -> round to 16 bit -> store s (saved for the
 //           backward) and accumulate (count, mean, M2) of the ROUNDED values per row (Chan's
 //           parallel update: no E[x^2] - E[x]^2 cancellation);
-//   merge   4 lanes of a row (shuffles) -> the 2-3 epilogue warps sharing the row (smem) ->
-//           barrier.cluster -> the 4 CTAs of the row (ld.shared::cluster) -> mean, rstd;
+//   merge   4 lanes of a row (shuffles) -> barrier.cluster -> the 4 CTAs of the row (ld.shared::cluster) -> mean, rstd;
 //   pass 2  re-read the CTA's own s (L2-hot, written by the same thread), normalise, scale, shift,
 //           store y.
 //
-// The mainloop is the 1-SM pipeline of gemm_kernel (TMA producer warp, one MMA-issuing lane, TMEM
-// accumulator); one 128 x BN tile per CTA (27 row tiles x 4 = 108 CTAs at C2 = one wave).
+// The mainloop is the pipeline of gemm_kernel (TMA producer warpgroup, two wgmma consumer
+// warpgroups with register accumulators); one 128 x BN tile per CTA.  A consumer warp owns 16 rows
+// x all BN columns of the tile, so a row's CTA-local statistics never leave the warp.
 #include "common.h"
 #include "gemm_impl.cuh"
 
@@ -38,18 +38,10 @@ constexpr float LN_FUSED_EPS = 1e-12f;
 
 template <int BN>
 struct GemmLnCfg {
-  static constexpr int B_TILE_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
-  static constexpr int STAGES = BN == 192 ? 4 : 3;
-  static constexpr int TMEM_COLS = 256;
-  static constexpr int EPI_SPLIT = epi_split(BN);          // warps sharing a TMEM lane quarter
-  static constexpr int EPI_WARPS = 4 * EPI_SPLIT;
-  static constexpr int THREADS = 128 + 32 * EPI_WARPS;
-  static constexpr int CHUNKS = BN / 32 / EPI_SPLIT;        // 32-column blocks per epilogue warp
   static constexpr int BAR_BYTES = 256;
-  static constexpr int EPI_STAGE_BYTES = EPI_WARPS * 32 * 33 * 4;
-  static constexpr int STAT_BYTES = (EPI_SPLIT + 2) * BM * 2 * 4;   // wstat[SPLIT] + cstat + fin
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + EPI_STAGE_BYTES + STAT_BYTES + 1024;
+  static constexpr int STAT_BYTES = BM * 2 * 4;                   // this CTA's (mean, M2) per row
+  static constexpr int SMEM_BYTES = GemmCfg<BN>::STAGES * GemmCfg<BN>::STAGE_BYTES + BAR_BYTES +
+                                    GemmCfg<BN>::EPI_STAGE_BYTES + STAT_BYTES + 1024;
 };
 
 // (na, ma, M2a) <- merge with (nb, mb, M2b)
@@ -68,26 +60,19 @@ __device__ __forceinline__ float2 ld_dsmem_f2(uint32_t cluster_addr) {
   return v;
 }
 
-__device__ __forceinline__ void epi_bar_sync(int nthreads) {
-  asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory");
-}
-
 template <int BN, bool kBF16, bool kDrop>
-__global__ void __launch_bounds__(GemmLnCfg<BN>::THREADS, 1)
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_ln_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const GemmParams p, const LnEpiParams q) {
-  using Cfg = GemmLnCfg<BN>;
+  using Cfg = GemmCfg<BN>;
   using T16 = typename Elem<kBF16>::T;
+  constexpr int CHUNKS = BN / 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-  float* epi_stage_base = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES);
-  float* wstat = epi_stage_base + Cfg::EPI_WARPS * 32 * 33;      // [EPI_SPLIT][128][2]
-  float* cstat = wstat + Cfg::EPI_SPLIT * BM * 2;                 // [128][2]  this CTA's (mean, M2) over BN columns
-  float* fin = cstat + BM * 2;                                    // [128][2]  (mean, rstd) of the whole row
+  float* epi_stage_base = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + GemmLnCfg<BN>::BAR_BYTES);
+  float* cstat = epi_stage_base + EPI_WARPS * 16 * EPI_PITCH;     // [128][2]  (mean, M2) over BN columns
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -99,110 +84,67 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);
     }
-    mbar_init(tmem_full_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
   pdl_launch_dependents();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
 
-  if (warp == 0) {
-    // ===================================================================== TMA producer
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-        uint8_t* sB = sA + A_TILE_BYTES;
-        mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-        tma_load_2d(sA, &tmA, &full_bar[stage], kb * BK, m0);
-        tma_load_2d(sB, &tmB, &full_bar[stage], kb * BK, n0);
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc(kBF16 ? 1 : 0, 0, 0, BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sA = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-        const uint32_t sB = sA + A_TILE_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)
-          umma_ss(tmem_base, umma_smem_desc(sA + k * 32, 16, 1024), umma_smem_desc(sB + k * 32, 16, 1024),
-                  idesc, (kb | k) != 0 ? 1u : 0u);
-        umma_commit(&empty_bar[stage]);
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(tmem_full_bar);
-    }
-  }
-
-  // ======================================================================= epilogue
   const bool is_epi = warp >= 4;
-  const int quarter = warp & 3;                 // TMEM lanes [32*quarter, +32) == tile rows
-  const int chalf = is_epi ? (warp - 4) >> 2 : 0;
+  const int cw = is_epi ? warp - 4 : 0;          // consumer warp: tile rows [16 cw, 16 cw + 16)
   const int sub_r = lane >> 2;
   const int cg = (lane & 3) * 8;
-  float* stage = epi_stage_base + (is_epi ? (warp - 4) : 0) * (32 * 33);
-  const int row_base = m0 + quarter * 32;
-  if (is_epi) {
+  float* stage = epi_stage_base + cw * (16 * EPI_PITCH);
+  const int row_base = m0 + 16 * cw;
+  float acc[BN / 2];
+  if (!is_epi) {
+    setmaxnreg_producer();
+    // ===================================================================== TMA producer
+    if (warp == 0 && lane == 0) {
+      int st = 0;
+      uint32_t phase = 0;
+      produce_tile<BN, false, false, 1>(smem, full_bar, empty_bar, &tmA, &tmB, m0, n0, 0, num_kb, st, phase, 0u);
+    }
+  } else {
+    setmaxnreg_consumer();
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int st = 0;
+    uint32_t phase = 0;
+    consume_tile<BN, false, false, kBF16, 1>(acc, smem, full_bar, empty_bar, num_kb, cw >> 2, st, phase, 0u);
     const DropoutRng rng = make_rng(p);
-    float cnt[4], mean[4], M2[4];
+    float cnt[2], mean[2], M2[2];
 #pragma unroll
-    for (int it = 0; it < 4; ++it) { cnt[it] = 0.f; mean[it] = 0.f; M2[it] = 0.f; }
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const uint32_t t_acc = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-#pragma unroll 1
-    for (int cw = 0; cw < Cfg::CHUNKS; ++cw) {
-      const int c = chalf * Cfg::CHUNKS + cw;
-      uint32_t r[32];
-      tmem_ld32(t_acc + c * 32, r);
+    for (int it = 0; it < 2; ++it) { cnt[it] = 0.f; mean[it] = 0.f; M2[it] = 0.f; }
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c) {
       const int col = n0 + c * 32 + cg;
-      // side inputs in the coalesced mapping, requested while the TMEM load is in flight
       const uint4 bias4 = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.bias) + col));
-      uint4 side[4];
+      uint4 side[2];
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
+      for (int it = 0; it < 2; ++it) {
         const int row = row_base + it * 8 + sub_r;
         side[it] = make_uint4(0, 0, 0, 0);
         if (row < p.M)
           side[it] = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.residual) +
                                                           static_cast<long long>(row) * p.ldr + col));
       }
-      tmem_ld_wait();
       __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 32; ++j) stage[lane * 33 + j] = __uint_as_float(r[j]);
+      stage_block<BN>(acc, c, lane, stage);
       __syncwarp();
       float bias8[8];
       unpack8_<kBF16>(bias4, bias8);
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
+      for (int it = 0; it < 2; ++it) {
         const int rr = it * 8 + sub_r;
         const int row = row_base + rr;
         float v[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = stage[rr * 33 + cg + i] + bias8[i];
+        for (int i = 0; i < 8; ++i) v[i] = stage[rr * EPI_PITCH + cg + i] + bias8[i];
         if (kDrop) {
           const uint64_t e = static_cast<uint64_t>(row) * static_cast<uint64_t>(p.N) + col;
           const uint4 rnd = rng.draw8(e >> 3);
@@ -227,13 +169,13 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         float q8 = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) { const float d = v[i] - m8; q8 = fmaf(d, d, q8); }
-        if (cw == 0) { cnt[it] = 8.f; mean[it] = m8; M2[it] = q8; }
+        if (c == 0) { cnt[it] = 8.f; mean[it] = m8; M2[it] = q8; }
         else chan_merge(cnt[it], mean[it], M2[it], 8.f, m8, q8);
       }
     }
     // the 4 lanes of a row (equal counts)
 #pragma unroll
-    for (int it = 0; it < 4; ++it) {
+    for (int it = 0; it < 2; ++it) {
 #pragma unroll
       for (int off = 1; off <= 2; off <<= 1) {
         const float mb = __shfl_xor_sync(0xffffffffu, mean[it], off);
@@ -241,29 +183,20 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         chan_merge(cnt[it], mean[it], M2[it], cnt[it], mb, qb);
       }
       if ((lane & 3) == 0) {
-        float* w = wstat + (chalf * BM + quarter * 32 + it * 8 + sub_r) * 2;
+        float* w = cstat + (16 * cw + it * 8 + sub_r) * 2;
         w[0] = mean[it];
         w[1] = M2[it];
       }
-    }
-    epi_bar_sync(Cfg::EPI_WARPS * 32);
-    if (chalf == 0) {                 // one thread per tile row: merge the warps that share it
-      const int rr = quarter * 32 + lane;
-      float n = static_cast<float>(32 * Cfg::CHUNKS), m = wstat[rr * 2], s2 = wstat[rr * 2 + 1];
-#pragma unroll
-      for (int h = 1; h < Cfg::EPI_SPLIT; ++h)
-        chan_merge(n, m, s2, static_cast<float>(32 * Cfg::CHUNKS), wstat[(h * BM + rr) * 2], wstat[(h * BM + rr) * 2 + 1]);
-      cstat[rr * 2] = m;
-      cstat[rr * 2 + 1] = s2;
     }
   }
   // ---- every CTA of the cluster has published its per-row partial statistics
   __syncwarp();
   cluster_sync_all();
   if (is_epi) {
-    if (chalf == 0) {
-      const int rr = quarter * 32 + lane;
-      const uint32_t local = smem_u32(cstat + rr * 2);
+    float mu[2], rs[2];
+#pragma unroll
+    for (int it = 0; it < 2; ++it) {
+      const uint32_t local = smem_u32(cstat + (16 * cw + it * 8 + sub_r) * 2);
       float n = 0.f, m = 0.f, s2 = 0.f;
 #pragma unroll
       for (int r4 = 0; r4 < LN_CLUSTER; ++r4) {
@@ -271,42 +204,32 @@ gemm_ln_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (r4 == 0) { n = static_cast<float>(BN); m = pr.x; s2 = pr.y; }
         else chan_merge(n, m, s2, static_cast<float>(BN), pr.x, pr.y);
       }
-      fin[rr * 2] = m;
-      fin[rr * 2 + 1] = rsqrtf(s2 * q.inv_n + LN_FUSED_EPS);
+      mu[it] = m;
+      rs[it] = rsqrtf(s2 * q.inv_n + LN_FUSED_EPS);
     }
-    epi_bar_sync(Cfg::EPI_WARPS * 32);
-    // ---- pass 2: y = (s - mean) * rstd * gamma + beta over this warp's columns
+    // ---- pass 2: y = (s - mean) * rstd * gamma + beta over this warp's rows
 #pragma unroll 1
-    for (int cw = 0; cw < Cfg::CHUNKS; ++cw) {
-      const int c = chalf * Cfg::CHUNKS + cw;
+    for (int c = 0; c < CHUNKS; ++c) {
       const int col = n0 + c * 32 + cg;
       float g8[8], b8[8];
       unpack8_<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(q.gamma) + col)), g8);
       unpack8_<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(q.beta) + col)), b8);
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const int rr = quarter * 32 + it * 8 + sub_r;
-        const int row = m0 + rr;
+      for (int it = 0; it < 2; ++it) {
+        const int row = row_base + it * 8 + sub_r;
         if (row >= p.M) continue;
         // own store of pass 1 (same thread, same address): a plain (coherent) load
         const uint4 s16 = *reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.out) +
                                                           static_cast<long long>(row) * p.ldo + col);
         float v[8];
         unpack8_<kBF16>(s16, v);
-        const float mu = fin[rr * 2], rs = fin[rr * 2 + 1];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = (v[i] - mu) * rs * g8[i] + b8[i];
+        for (int i = 0; i < 8; ++i) v[i] = (v[i] - mu[it]) * rs[it] * g8[i] + b8[i];
         store8<kBF16>(q.y, static_cast<long long>(row) * q.ldy + col, v);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
   cluster_sync_all();      // nobody exits while a peer may still read its statistics
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
 }
 
 template <int BN, bool kBF16, bool kDrop>
@@ -319,7 +242,7 @@ static int launch_gemm_ln_t(const GemmParams& p, const LnEpiParams& q, const CUt
     UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   const int grid = p.tiles_m * LN_CLUSTER;
   ProfScope ps(stream);
-  UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, LN_CLUSTER, tmA,
+  UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, LN_CLUSTER, tmA,
                            tmB, p, q));
   return 0;
 }

@@ -4,7 +4,7 @@
 
 namespace ub {
 
-constexpr int BM = 128;   // accumulator rows per CTA == TMEM lanes
+constexpr int BM = 128;   // accumulator rows per CTA (two consumer warpgroups of 64)
 constexpr int BK = 64;    // 64 x 16-bit = one 128-byte swizzle row
 
 struct GemmParams {

@@ -22,11 +22,11 @@
 // (wrong data, but never a hung GPU); the host checks the word.
 //
 // Three forms of the same protocol (ub200_peer_allreduce_args.max_ctas), in the order they were built;
-// the measurements that decided between them are in DESIGN.md §6:
+//
 //   > 0  peer_allreduce_kernel: ONE persistent kernel, both phases with SM loads / posted remote stores.
 //        256 threads x <= 64 registers, no shared memory, so a CTA fits next to a persistent GEMM CTA
-//        (512 x 80-96 registers) — but 16 K registers hold only ~32 KB in flight: 148 CTAs reach
-//        590 GB/s (algorithmic, 2 ranks), 32 CTAs 205 GB/s.
+//        (384 x <= 168 registers) — but 16 K registers hold only ~32 KB in flight, so it needs most
+//        of the SMs to approach NVLink bandwidth.
 //   = 0  peer_push_kernel + peer_reduce_kernel: work-sized grids of short-lived CTAs.
 //   < 0  (default) the COPY ENGINES move the bytes (cudaMemcpyAsync nodes), peer_sync_kernel runs the
 //        barriers, peer_reduce_local_kernel reduces out of local HBM: nothing competes with the
@@ -322,8 +322,8 @@ __global__ void __launch_bounds__(256, 4) peer_reduce_kernel(const PeerParams p)
 
 // ------------------------------------------------------------------------------------------------
 // Form 3 (max_ctas < 0), the default: the COPY ENGINES move the bytes, the SMs only reduce.
-// Measured on 2 x B200 (profiles/r02_k_*): with either SM form the step takes the same 4.15 ms whether
-// the exchange is issued slice by slice during the backward or once after it — exchange CTAs that are
+// With either SM form, issuing the exchange slice by slice during the backward gains little over
+// issuing it once after the backward — exchange CTAs that are
 // scheduled ahead of the backward's CTAs stall it, exchange CTAs scheduled behind them do not run
 // until it is over.  So the SMs are taken out of the data path:
 //   A  (world-1) cudaMemcpyAsync nodes: my sub-slice q  ->  stage_q[rank]          (DMA over NVLink)
@@ -477,7 +477,12 @@ int ub200_peer_allreduce(const ub200_peer_allreduce_args* a, ub200_stream_t stre
                "peer_allreduce: staging buffer too small (%lld < %lld bytes)", (long long)a->stage_bytes,
                (long long)(per * a->world * 16));
   p.scale = a->scale;
-  p.timeout_cycles = a->timeout_ms > 0 ? static_cast<long long>(a->timeout_ms) * 1900000ll : 38000000000ll;
+  // flag waits count SM clocks: convert at the device's maximum SM clock (a slower clock only
+  // lengthens the bound)
+  int clock_khz = 0, dev = 0;
+  UB_CHECK_CUDA(cudaGetDevice(&dev));
+  UB_CHECK_CUDA(cudaDeviceGetAttribute(&clock_khz, cudaDevAttrClockRate, dev));
+  p.timeout_cycles = static_cast<long long>(a->timeout_ms > 0 ? a->timeout_ms : 20000) * clock_khz;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (a->max_ctas < 0) {
     // form 3: copy engines for the NVLink transfers, SMs for the flags and the local reduction

@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05
-// (alloc / mma / commit / ld), UMMA shared-memory + instruction descriptors.
-// Everything here is hand-written for B200; there is no fallback path.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor, with cluster
+// multicast), clusters, wgmma shared-memory descriptors.  The wgmma instructions themselves are
+// in wgmma.cuh.  Everything here is hand-written for H100; there is no fallback path.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -78,14 +78,8 @@ __device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
 
 // ---------------------------------------------------------------- fences
 __device__ __forceinline__ void fence_proxy_async_smem() {
-  // make generic-proxy smem writes visible to the async proxy (UMMA / TMA reads)
+  // make generic-proxy smem writes visible to the async proxy (wgmma / TMA reads)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -104,17 +98,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// 2-D tiled load issued by either CTA of a cta_group::2 pair: the tile lands in the ISSUING
-// CTA's smem, the transaction bytes are counted on `bar_cluster_addr` — a shared::cluster
-// address, normally the LEADER CTA's full barrier (see mapa_shared).
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m,
-                                                uint32_t bar_cluster_addr, int c0, int c1) {
+// 2-D tiled load multicast to the CTAs of `cta_mask` in the cluster: the tile lands at the same
+// shared-memory offset in each of them and completes on the mbarrier at the same offset there.
+__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
+                                               int c0, int c1, uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
       :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0),
-        "r"(c1)
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0),
+        "r"(c1), "h"(cta_mask)
       : "memory");
 }
 
@@ -141,121 +134,18 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// ---------------------------------------------------------------- TMEM alloc
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor, 128-byte swizzle (layout_type = 2), Blackwell version = 1.
+// ---------------------------------------------------------------- wgmma descriptors
+// Shared-memory matrix descriptor, 128-byte swizzle (layout type 1 in bits [62,64)).
 //   K-major  tile: rows of 128 B (64 x 16-bit along K); 8-row groups 1024 B apart (SBO).
 //   MN-major tile: rows of 128 B (64 x 16-bit along M/N), one row per K index; 8-K groups
 //                  1024 B apart (SBO); 64-wide M/N groups `lbo_bytes` apart (LBO).
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);              // [0,14)  start address
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;     // [16,30) leading byte offset
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;     // [32,46) stride byte offset
-  d |= static_cast<uint64_t>(1) << 46;                              // [46,48) version = 1
-  d |= static_cast<uint64_t>(2) << 61;                              // [61,64) SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                              // SWIZZLE_128B
   return d;
-}
-
-// Instruction descriptor for tcgen05.mma.kind::f16 with fp32 accumulation.
-//   fmt: 0 = fp16 operands, 1 = bf16 operands.  a_mn / b_mn: 1 = MN-major operand.
-__host__ __device__ constexpr uint32_t umma_idesc(int fmt, int a_mn, int b_mn, int M, int N) {
-  return (1u << 4)                                   // c_format = F32
-         | (static_cast<uint32_t>(fmt) << 7)         // a_format
-         | (static_cast<uint32_t>(fmt) << 10)        // b_format
-         | (static_cast<uint32_t>(a_mn) << 15)       // a_major
-         | (static_cast<uint32_t>(b_mn) << 16)       // b_major
-         | (static_cast<uint32_t>(N >> 3) << 17)     // n_dim
-         | (static_cast<uint32_t>(M >> 4) << 24);    // m_dim
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread on behalf of the CTA.
-__device__ __forceinline__ void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                        uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// cta_group::2: one thread of the LEADER CTA issues an M=256 MMA for the CTA pair; each CTA
-// supplies its own 128 A rows and its own half of the B rows from the same smem offsets and
-// receives its 128 accumulator rows in its own TMEM.
-__device__ __forceinline__ void umma_ss_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// completion of the pair's MMAs -> arrive on the mbarrier at this offset in every CTA of cta_mask
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// ---------------------------------------------------------------- TMEM -> registers
-// 32 lanes x 32 consecutive fp32 columns: thread t of warp w gets lane (32*(w%4)+t).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 // ---------------------------------------------------------------- 16-bit storage types
@@ -352,10 +242,9 @@ __device__ __forceinline__ float rcp_approx(float x) {
 // t = 1/(1 + p|x|/sqrt2)  (Abramowitz & Stegun 7.1.26, |abs err| <= 1.5e-7 — far below the
 // 16-bit output rounding).  `ex` returns exp(-x^2/2), shared with the pdf in the derivative.
 // The reciprocal and the exponential are the bare MUFU approximations (rcp.approx.ftz on an
-// argument >= 1, ex2.approx.ftz on x^2 * -log2(e)/2): ncu on the FFN1 GEMM showed 39 issued
-// instructions per output element with __fdividef / __expf — their range-handling FSETP / FMUL /
-// branch sequences — in an epilogue that is issue-bound (2 warps per scheduler, 46 % issue
-// utilisation, tensor pipe 30 % active).
+// argument >= 1, ex2.approx.ftz on x^2 * -log2(e)/2), without the range-handling FSETP / FMUL /
+// branch sequences __fdividef / __expf add: the GELU epilogues run once per output element and
+// compete for issue slots with the rest of the epilogue.
 __device__ __forceinline__ float normal_cdf(float x, float& ex) {
   const float ax = fabsf(x) * 0.70710678118654752440f;
   const float t = rcp_approx(fmaf(0.3275911f, ax, 1.0f));

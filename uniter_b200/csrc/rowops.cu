@@ -270,7 +270,7 @@ ln_bwd_kernel(const LnBwdParams p) {
     }
     __syncthreads();
     // 64 threads x 4 consecutive columns: one 16-byte vector atomic per quantity instead of four
-    // scalar ones (the column-sum atomics of 148 CTAs were ~1/3 of this kernel's time)
+    // scalar ones (one column-sum atomic per 4 columns instead of one per column)
     if (threadIdx.x < 64) {
       const int c4 = threadIdx.x * 4;
       const int col = c4 + i * 256;
@@ -293,7 +293,7 @@ ln_bwd_kernel(const LnBwdParams p) {
 // ------------------------------------------------------------------------------ LayerNorm bwd, split form
 // The fused kernel above keeps 3 x NV x 8 column accumulators per thread (240 registers at H = 768:
 // one CTA of 8 warps per SM) and every warp walks through a serial chain of 3 warp reductions per
-// row, so it runs at ~0.2 of the HBM roofline (ncu: 15 us for 21 MB).  Split form, for the plain case
+// row, so it runs far below the HBM roofline.  Split form, for the plain case
 // (no row-kind mask, dropout on the Linear branch):
 //   ln_bwd_rows_kernel  one warp per row, nothing carried between rows (~90 registers: several CTAs
 //                       per SM): dx, the dropout-masked copy, and (mean, rstd) of the row to `stats`;

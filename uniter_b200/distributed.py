@@ -1,4 +1,4 @@
-"""Data-parallel plumbing over torch.distributed (NCCL on B200 / NVLink 5; gloo for CPU tests).
+"""Data-parallel plumbing over torch.distributed (NCCL on H100 / NVLink 4; gloo for CPU tests).
 
 Replaces the Horovod path of the reference (utils/distributed.py):
   * `all_reduce_and_rescale_tensors(grads, 1.0)` (:16-43; call sites train_vqa.py:193-199,
@@ -160,8 +160,8 @@ class GradientReducer:
         of the earlier layers still runs; only the embedding front-end slice is reduced after the
         backward.  `sm_reserve` > 0: during that overlap the library's persistent kernels leave
         `sm_reserve` SMs to the collective, and the collective runs on a communicator capped to the
-        same number of CTAs (must be called by all ranks).  Measured on 2 x B200 (C2,
-        profiles/r01_scale2_variants.json): reserving SMs cost more than it saved, hence default 0.
+        same number of CTAs (must be called by all ranks).  Default 0: reserving SMs
+        costs the backward more than it gains the collective.
         `transport` "peer": the slices are exchanged by the library's own NVLink peer-memory kernel
         (PeerExchange; `peer_ctas` / `peer_tail_ctas` select its form for the slices shipped while the
         backward runs / after it: < 0 copy engines + local reduction, 0 short-lived CTAs, > 0 one persistent

@@ -6,7 +6,7 @@ Parameter names and module trees follow the reference so its checkpoints load
 * ``UniterForMLM`` — the MLM branch of ``UniterForPretraining`` (model/pretrain.py:50-60,
   107-133).  SURVEY.md §8f-1: the head runs on libub200 — masked rows are gathered straight from
   the PACKED encoder output, ``BertPredictionHeadTransform`` (model/layer.py:188-203) is the
-  tcgen05 GEMM with the bias+GELU epilogue + the LayerNorm kernel, the tied decoder
+  wgmma GEMM with the bias+GELU epilogue + the LayerNorm kernel, the tied decoder
   (model/layer.py:206-222) is the same GEMM over the un-padded [V, H] embedding table
   (``n_valid``), and the cross-entropy is one fused kernel per direction; the decoder's dgrad
   (few output tiles, K = V = 28996) runs split-K.

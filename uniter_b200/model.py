@@ -1,4 +1,4 @@
-"""Drop-in `UniterModel` for ChenRocks/UNITER running the encoder on libub200 (sm_100a).
+"""Drop-in `UniterModel` for ChenRocks/UNITER running the encoder on libub200 (sm_90a).
 
 Mirrors the reference's Python contract for the hot path (SURVEY.md §8b-B1):
 
@@ -12,7 +12,7 @@ Mirrors the reference's Python contract for the hot path (SURVEY.md §8b-B1):
 What differs underneath: the encoder stack runs over PACKED valid tokens ([T, H], no padding
 compute) through hand-written CUDA kernels behind a C ABI; rows where ``attention_mask == 0`` are
 returned as zeros (the reference returns garbage there that no head reads).  There is no
-CPU / eager fallback: parameters must be fp16 or bf16 and live on a B200.
+CPU / eager fallback: parameters must be fp16 or bf16 and live on an H100.
 """
 import copy
 import ctypes as C
@@ -210,7 +210,7 @@ class BertLayer(nn.Module):
 
 class BertPooler(nn.Module):
     """tanh(dense(x[:, 0])) — model/layer.py:173-185 — on libub200: the [CLS] rows are read in place
-    from the [B, L, H] tensor (row pitch L*H), one tcgen05 GEMM with the bias + tanh epilogue."""
+    from the [B, L, H] tensor (row pitch L*H), one wgmma GEMM with the bias + tanh epilogue."""
 
     def __init__(self, config):
         super().__init__()
@@ -468,7 +468,7 @@ class LibLinear(torch.autograd.Function):
     """y = act(x W^T + b) with W [N, K] (an nn.Linear weight, `w_kn` False), or y = act(x W + b) with
     W [K, N] (`w_kn` True: the reference's `F.linear(h, weight.t(), bias)` of RegionFeatureRegression,
     model/pretrain.py:29-32, whose weight is the tied img_linear.weight) — forward, dgrad and wgrad on
-    the tcgen05 GEMM (operands read un-transposed in every direction), bias gradient by ub200_colsum.
+    the wgmma GEMM (operands read un-transposed in every direction), bias gradient by ub200_colsum.
     act = tanh when `tanh` (BertPooler).  N may be any size (padded to 8 internally: ITM's 2
     classes, the 1601 region labels).  Parameters that live in a gradient arena get their gradients
     written there directly (None is returned to autograd); others are returned normally."""
@@ -591,7 +591,7 @@ class _EmbedFront(torch.autograd.Function):
             _lib.check(lib.ub200_embed_gather_cast(
                 img_feat.data_ptr(), 1 if img_feat.dtype == torch.float32 else 0, idx[4].data_ptr(),
                 idx[5].data_ptr(), mask_row.data_ptr(), A.data_ptr(), T, D, dt, stream))
-            G = ops.gemm(A, ie.img_linear.weight, bias=ie.img_linear.bias)   # img_linear on the tcgen05 core
+            G = ops.gemm(A, ie.img_linear.weight, bias=ie.img_linear.bias)   # img_linear on the wgmma core
             pos_feat = img_pos_feat.float().contiguous().view(-1, img_pos_feat.size(-1))
             assert pos_feat.size(1) == 7
         x = torch.empty(T, H, device=dev, dtype=dtype)
@@ -620,7 +620,7 @@ class _EmbedFront(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dx):
-        """Row-kind masked LayerNorm backward (x4), img_linear wgrad on the tcgen05 GEMM, then the
+        """Row-kind masked LayerNorm backward (x4), img_linear wgrad on the wgmma GEMM, then the
         table gradients in three launches (ub200_embed_bwd_scatter / _colsums); every small fp32
         gradient lives in ONE staging buffer whose layout equals the arena's front-end small section,
         so one launch converts (or accumulates) all of them into the parameters' .grad views."""

@@ -16,7 +16,7 @@ def gemm(a, b, *, a_major=0, b_major=0, bias=None, residual=None, aux=None, out=
          gelu=False, dgelu=False, accumulate=False, out_fp32=False, colsum=None,
          dropout_p=0.0, rng_seed=0, rng_stream=0, tile_n=0, max_ctas=0, cluster=0, k_splits=0,
          n_valid=0, rng_offset_dev=None, tanh=False, ln=None, _debug_flags=0):
-    """D = epilogue(A . B^T) on the tcgen05 GEMM core.  Returns `out` (and pre-activation if gelu).
+    """D = epilogue(A . B^T) on the wgmma GEMM core.  Returns `out` (and pre-activation if gelu).
 
     a: [M,K] (a_major=0) or [K,M] (a_major=1);  b: [N,K] (b_major=0) or [K,N] (b_major=1).
     ln=(gamma, beta): fused residual + LayerNorm epilogue — returns (s, LayerNorm(s)); needs bias and

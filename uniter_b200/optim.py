@@ -1,6 +1,6 @@
 """Fused multi-tensor AdamW with fp32 master weights on libub200 (SURVEY.md §8f-2).
 
-Replaces, for 16-bit models on a B200, what the reference assembles from three pieces:
+Replaces, for 16-bit models on an H100, what the reference assembles from three pieces:
 
 * ``optim/adamw.py:43-103`` — the AdamW update itself (bias-corrected step size; decoupled weight
   decay ``p -= lr * wd * p`` applied AFTER the Adam update);
