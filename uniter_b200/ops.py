@@ -94,14 +94,24 @@ def gemm(a, b, *, a_major=0, b_major=0, bias=None, residual=None, aux=None, out=
     return (out, out2) if gelu else out
 
 
+def _out_buffer(buf, shape, like, dtype):
+    """`buf` checked as a contiguous output of `shape` / `dtype` on like's device, or a new one."""
+    if buf is None:
+        return torch.empty(shape, device=like.device, dtype=dtype)
+    assert tuple(buf.shape) == tuple(shape) and buf.dtype == dtype and buf.is_contiguous() \
+        and buf.device == like.device, "output buffer must be a contiguous %s %s" % (dtype, tuple(shape))
+    return buf
+
+
 def attn_fwd(qkv, cu_seqlens, max_seqlen, num_heads, dropout_p=0.0, rng_seed=0, rng_stream=0,
-             rng_offset_dev=None):
-    """ctx [T, H], lse [heads, T] = fused varlen attention over packed qkv [T, 3H]."""
+             rng_offset_dev=None, ctx=None, lse=None):
+    """ctx [T, H], lse [heads, T] = fused varlen attention over packed qkv [T, 3H].
+    ctx / lse: optional preallocated outputs (written, not accumulated into)."""
     lib = _lib.load()
     T, H3 = qkv.shape
     H = H3 // 3
-    ctx = torch.empty(T, H, device=qkv.device, dtype=qkv.dtype)
-    lse = torch.empty(num_heads, T, device=qkv.device, dtype=torch.float32)
+    ctx = _out_buffer(ctx, (T, H), qkv, qkv.dtype)
+    lse = _out_buffer(lse, (num_heads, T), qkv, torch.float32)
     a = _lib.AttnArgs(qkv=qkv.data_ptr(), ctx=ctx.data_ptr(), lse=lse.data_ptr(),
                       cu_seqlens=cu_seqlens.data_ptr(), batch=cu_seqlens.numel() - 1,
                       total_tokens=T, max_seqlen=max_seqlen, hidden=H, num_heads=num_heads,
@@ -112,11 +122,13 @@ def attn_fwd(qkv, cu_seqlens, max_seqlen, num_heads, dropout_p=0.0, rng_seed=0, 
 
 
 def attn_bwd(qkv, ctx, lse, dctx, cu_seqlens, max_seqlen, num_heads, dropout_p=0.0, rng_seed=0,
-             rng_stream=0, dbias=None, rng_offset_dev=None):
+             rng_stream=0, dbias=None, rng_offset_dev=None, dqkv=None):
+    """dqkv [T, 3H] of attn_fwd; dbias [3H] fp32, if given, is accumulated into (column sums of dqkv).
+    dqkv: optional preallocated output (written, not accumulated into)."""
     lib = _lib.load()
     T, H3 = qkv.shape
     H = H3 // 3
-    dqkv = torch.empty_like(qkv)
+    dqkv = _out_buffer(dqkv, (T, H3), qkv, qkv.dtype)
     ws_bytes = lib.ub200_attn_bwd_workspace_bytes(T, H, max_seqlen)
     ws = torch.empty(max(ws_bytes, 1), device=qkv.device, dtype=torch.uint8)
     a = _lib.AttnArgs(qkv=qkv.data_ptr(), ctx=ctx.data_ptr(), lse=lse.data_ptr(),
