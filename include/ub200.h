@@ -445,6 +445,36 @@ int ub200_adamw_step(const ub200_adam_segment* segs_dev, const int32_t* blk_star
                      float max_norm, const float* sumsq, const ub200_adam_state* state_dev,
                      const float* lr_dev, ub200_stream_t stream);
 
+/* Device-resident dynamic loss scaling (apex amp's LossScaler in dynamic mode, train_vqa.py:152,189-199;
+ * pre-training keeps one scaler per task, pretrain.py:230-233,298-301): a table of entries, one per
+ * loss id, in DEVICE memory at a fixed address.  The caller multiplies its loss by `scale` on the
+ * device before the backward; ub200_adam_prep_scaled (instead of ub200_adam_prep, after
+ * ub200_grad_sumsq) sets found_inf / step / skipped exactly as ub200_adam_prep does, records
+ * inv_scale = 1 / scale (what this step's gradients carry), then updates entry `loss_id` only:
+ *   overflow:  scale = max(scale / 2, min_scale) (plain scale / 2 when min_scale <= 0), unskipped = 0
+ *   otherwise: unskipped += 1; when unskipped == window: scale = min(scale * 2, max_scale), unskipped = 0
+ * ub200_adamw_step_scaled is ub200_adamw_step in device-state mode with the unscale factor read from
+ * the entry's inv_scale (gradient multiplier and clip norm alike).  No host read anywhere: a whole
+ * fp16 step, loss scale included, replays from one CUDA graph.  apex defaults: scale 2^16,
+ * window 2000, max_scale 2^24, no floor.  loss_id must index the caller's table.  The prep kernel is
+ * an ordinary launch with full dependencies on ub200_grad_sumsq before it and ub200_adamw_step_scaled
+ * after it (not a programmatic dependent), so the overflow check holds inside captured graphs. */
+typedef struct {
+  float scale;        /* current loss scale */
+  int32_t unskipped;  /* clean steps since the scale last changed */
+  float inv_scale;    /* 1 / scale of the step the last ub200_adam_prep_scaled ran for */
+  int32_t window;     /* clean steps before the scale doubles (apex scale_seq_len) */
+  float max_scale;    /* growth cap */
+  float min_scale;    /* floor on overflow; <= 0: none */
+  int32_t _pad[2];
+} ub200_loss_scaler;
+int ub200_adam_prep_scaled(const float* sumsq, ub200_adam_state* state_dev, ub200_loss_scaler* scalers_dev,
+                           int32_t loss_id, ub200_stream_t stream);
+int ub200_adamw_step_scaled(const ub200_adam_segment* segs_dev, const int32_t* blk_start_dev, int32_t nseg,
+                            int32_t nblocks, float beta1, float beta2, float eps, float max_norm,
+                            const float* sumsq, const ub200_adam_state* state_dev, const float* lr_dev,
+                            const ub200_loss_scaler* scalers_dev, int32_t loss_id, ub200_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Gradient exchange over NVLink peer memory — replaces utils/distributed.py:16-43
  * (all_reduce_and_rescale_tensors: flatten -> hvd.allreduce_ = mean over ranks -> unflatten; call

@@ -96,6 +96,12 @@ class AdamSegment(C.Structure):
                 ("flags", C.c_int32)]
 
 
+class LossScalerEntry(C.Structure):
+    _fields_ = [("scale", C.c_float), ("unskipped", C.c_int32), ("inv_scale", C.c_float),
+                ("window", C.c_int32), ("max_scale", C.c_float), ("min_scale", C.c_float),
+                ("_pad", C.c_int32 * 2)]
+
+
 MAX_PEERS = 8
 
 
@@ -180,6 +186,12 @@ def load():
                                      C.c_void_p]
     lib.ub200_adam_prep.restype = C.c_int
     lib.ub200_adam_prep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.ub200_adam_prep_scaled.restype = C.c_int
+    lib.ub200_adam_prep_scaled.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]
+    lib.ub200_adamw_step_scaled.restype = C.c_int
+    lib.ub200_adamw_step_scaled.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_float,
+                                            C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_int32, C.c_void_p]
     lib.ub200_gather_rows.restype = C.c_int
     lib.ub200_gather_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.ub200_peer_flags_bytes.restype = C.c_int64

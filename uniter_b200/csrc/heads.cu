@@ -215,16 +215,45 @@ struct AdamHyper {
   const float* sumsq;     // device scalar from sumsq_kernel (of the SCALED gradients) or NULL
   const ub200_adam_state* state;   // device-resident step counter / overflow flag, or NULL (legacy)
   const float* lr;                 // per-group learning rates (device), with `state`
+  const ub200_loss_scaler* scaler; // non-NULL: inv_scale is read from scaler->inv_scale instead
 };
+
+__device__ __forceinline__ bool sumsq_finite(float s) { return (s == s) && (fabsf(s) <= 3.0e38f); }
 
 // found_inf / step bookkeeping on the device (one thread), between sumsq_kernel and adamw_kernel
 __global__ void adam_prep_kernel(const float* __restrict__ sumsq, ub200_adam_state* __restrict__ st) {
   pdl_launch_dependents();
   pdl_wait();
-  const float s = *sumsq;
-  const bool finite = (s == s) && (fabsf(s) <= 3.0e38f);
+  const bool finite = sumsq_finite(*sumsq);
   st->found_inf = finite ? 0 : 1;
   if (finite) st->step += 1; else st->skipped += 1;
+}
+
+// adam_prep_kernel + apex's dynamic LossScaler.update_scale for the scaler entry of this step's loss:
+// records the unscale factor of the gradients (1 / the scale their loss was multiplied by), then
+// halves the scale on overflow (down to the optional floor) or doubles it after `window` clean steps
+// (up to max_scale).  Only `sc` moves: the entries of the other losses are not touched.
+// No griddepcontrol here (see ub200_adam_prep_scaled): launched behind sumsq_kernel with a full
+// dependency, and never triggering early, so adamw_kernel can only start once it has finished.
+__global__ void adam_prep_scaled_kernel(const float* __restrict__ sumsq, ub200_adam_state* __restrict__ st,
+                                        ub200_loss_scaler* __restrict__ sc) {
+  const bool finite = sumsq_finite(*sumsq);
+  st->found_inf = finite ? 0 : 1;
+  if (finite) st->step += 1; else st->skipped += 1;
+  const float scale = sc->scale;
+  sc->inv_scale = 1.0f / scale;
+  if (!finite) {
+    const float halved = scale * 0.5f;
+    sc->scale = sc->min_scale > 0.f ? fmaxf(halved, sc->min_scale) : halved;
+    sc->unskipped = 0;
+  } else {
+    int32_t u = sc->unskipped + 1;
+    if (u == sc->window) {
+      sc->scale = fminf(scale * 2.0f, sc->max_scale);
+      u = 0;
+    }
+    sc->unskipped = u;
+  }
 }
 
 __global__ void __launch_bounds__(256)
@@ -250,10 +279,11 @@ adamw_kernel(const ub200_adam_segment* __restrict__ segs, const int* __restrict_
     }
     lr_wd = lr * sg.weight_decay;
   }
-  float gmul = h.inv_scale;
+  const float inv_scale = h.scaler != nullptr ? h.scaler->inv_scale : h.inv_scale;
+  float gmul = inv_scale;
   if (h.max_norm > 0.f && h.sumsq != nullptr) {
     // torch.nn.utils.clip_grad_norm_: coef = max_norm / (total_norm + 1e-6), applied iff < 1
-    const float total = sqrtf(__ldg(h.sumsq)) * h.inv_scale;
+    const float total = sqrtf(__ldg(h.sumsq)) * inv_scale;
     const float coef = h.max_norm / (total + 1e-6f);
     if (coef < 1.f) gmul *= coef;
   }
@@ -433,7 +463,44 @@ extern "C" int ub200_adamw_step(const ub200_adam_segment* segs_dev, const int32_
                "adamw_step: invalid hyper-parameters");
   UB_CHECK_ARG(max_norm <= 0.f || sumsq, "adamw_step: clipping needs the sumsq scalar");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  AdamHyper h{beta1, beta2, eps, inv_scale, max_norm, sumsq, state_dev, lr_dev};
+  AdamHyper h{beta1, beta2, eps, inv_scale, max_norm, sumsq, state_dev, lr_dev, nullptr};
+  ProfScope ps(stream);
+  UB_CHECK_CUDA(launch_pdl(adamw_kernel, dim3(nblocks), dim3(256), 0, stream, 1, segs_dev, blk_start_dev,
+                           nseg, h));
+  return 0;
+}
+
+extern "C" int ub200_adam_prep_scaled(const float* sumsq, ub200_adam_state* state_dev,
+                                      ub200_loss_scaler* scalers_dev, int32_t loss_id, ub200_stream_t stream_) {
+  using namespace ub;
+  UB_CHECK_ARG(sumsq && state_dev && scalers_dev, "adam_prep_scaled: null pointer");
+  UB_CHECK_ARG(loss_id >= 0, "adam_prep_scaled: loss_id must be >= 0");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ProfScope ps(stream);
+  // An ordinary launch, not a programmatic dependent of sumsq_kernel: inside a captured CUDA graph the
+  // PDL-chained form was measured reading the sum of squares before sumsq_kernel had added the
+  // non-finite part of it (an overflowed step counted as clean), and adamw_kernel, when this kernel
+  // triggered its dependents early, reading a stale found_inf.  Full dependencies on both sides cost
+  // one launch latency each per step.
+  adam_prep_scaled_kernel<<<1, 1, 0, stream>>>(sumsq, state_dev, scalers_dev + loss_id);
+  UB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int ub200_adamw_step_scaled(const ub200_adam_segment* segs_dev, const int32_t* blk_start_dev,
+                                       int32_t nseg, int32_t nblocks, float beta1, float beta2, float eps,
+                                       float max_norm, const float* sumsq, const ub200_adam_state* state_dev,
+                                       const float* lr_dev, const ub200_loss_scaler* scalers_dev,
+                                       int32_t loss_id, ub200_stream_t stream_) {
+  using namespace ub;
+  UB_CHECK_ARG(segs_dev && blk_start_dev && nseg > 0 && nblocks > 0, "adamw_step_scaled: bad argument");
+  UB_CHECK_ARG(state_dev && lr_dev && scalers_dev && loss_id >= 0,
+               "adamw_step_scaled: needs state_dev, lr_dev, scalers_dev and loss_id >= 0");
+  UB_CHECK_ARG(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f,
+               "adamw_step_scaled: invalid hyper-parameters");
+  UB_CHECK_ARG(max_norm <= 0.f || sumsq, "adamw_step_scaled: clipping needs the sumsq scalar");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  AdamHyper h{beta1, beta2, eps, 1.0f, max_norm, sumsq, state_dev, lr_dev, scalers_dev + loss_id};
   ProfScope ps(stream);
   UB_CHECK_CUDA(launch_pdl(adamw_kernel, dim3(nblocks), dim3(256), 0, stream, 1, segs_dev, blk_start_dev,
                            nseg, h));

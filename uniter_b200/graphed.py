@@ -44,7 +44,7 @@ class _Bucket(object):
 class GraphedStep(object):
     def __init__(self, module, loss_fn, token_bucket=128, reducer=None, optimizer=None,
                  optimizer_kwargs=None, zero_all_grads=False, mask_key="attn_masks", warmup=2,
-                 reducer_mode="split"):
+                 reducer_mode="split", loss_scaler=None, loss_ids=None):
         """module: the root nn.Module (its parameters' gradients go to one arena);
         loss_fn(batch_on_device) -> scalar loss (runs the forward);
         reducer: optional GradientReducer.  reducer_mode "split" (default): the step is captured as a
@@ -58,7 +58,14 @@ class GraphedStep(object):
         executed collectives the other ranks did not take part in (fixed: captures are local now), and
         were not re-measured since.
         optimizer: optional FusedAdamW stepped inside the (tail) graph; zero_all_grads: see
-        GradArena.begin_step(zero_all=...)."""
+        GradArena.begin_step(zero_all=...).
+        loss_scaler: optional DynamicLossScaler (fp16): the step back-propagates
+        loss_scaler.scale(loss, id) and the optimizer unscales by, and updates, entry `id` — all from
+        device memory, so replays follow the current scale and a change of scale never re-captures;
+        the returned loss stays unscaled.  loss_ids: {tag: id} (e.g. one scaler per pre-training task,
+        pretrain.py:230-233); without it every step uses id 0."""
+        if loss_scaler is not None and "grad_scale" in (optimizer_kwargs or {}):
+            raise ValueError("GraphedStep: give either loss_scaler or optimizer_kwargs['grad_scale'], not both")
         self.module = module
         self.loss_fn = loss_fn
         self.token_bucket = int(token_bucket)
@@ -66,6 +73,8 @@ class GraphedStep(object):
         self.reducer_mode = reducer_mode if reducer is not None else "none"
         self.optimizer = optimizer
         self.optimizer_kwargs = optimizer_kwargs or {}
+        self.loss_scaler = loss_scaler
+        self.loss_ids = dict(loss_ids) if loss_ids is not None else None
         self.zero_all = bool(zero_all_grads)
         self.mask_key = mask_key
         self.warmup = int(warmup)
@@ -81,13 +90,23 @@ class GraphedStep(object):
         self.captures = 0
 
     # ------------------------------------------------------------------ keys / buffers
-    def _key(self, host_batch, lens, accumulate, tag=None):
+    def _key(self, host_batch, lens, accumulate, tag=None, step_optimizer=True):
         T = int(sum(lens))
         T_pad = max(_round_up(T, self.token_bucket), self.token_bucket)
         maxseq = _round_up(max(max(lens), 1, T_pad - T), 128)
         sig = tuple((k, tuple(v.shape), str(v.dtype)) for k, v in sorted(host_batch.items())
                     if torch.is_tensor(v))
-        return (sig, T_pad, maxseq, bool(accumulate), tag), T_pad, maxseq
+        return (sig, T_pad, maxseq, bool(accumulate), tag, self._steps_optimizer(step_optimizer)), T_pad, maxseq
+
+    def _steps_optimizer(self, step_optimizer):
+        return self.optimizer is not None and bool(step_optimizer)
+
+    def _loss_id(self, tag):
+        if self.loss_ids is None:
+            return 0
+        if tag not in self.loss_ids:
+            raise KeyError("GraphedStep: no loss id for tag %r (loss_ids has %s)" % (tag, sorted(self.loss_ids)))
+        return int(self.loss_ids[tag])
 
     def _fill_meta(self, bk, lens, L):
         """Packing bookkeeping of this batch -> the bucket's static device buffer (one H2D)."""
@@ -104,26 +123,34 @@ class GraphedStep(object):
         return offs
 
     # ------------------------------------------------------------------ the captured region
-    def _run(self, bk, accumulate, tag=None):
+    def _run(self, bk, accumulate, tag=None, step_optimizer=True):
         self.rng_counter.add_(64)                       # fresh dropout masks for this replay
         self.arena.begin_step(accumulate=accumulate, zero_all=self.zero_all)
         _model._RNG_GRAPH["dev"] = self.rng_counter
         _model._RNG_GRAPH["call"] = 0
         try:
             loss = self.loss_fn(bk.inputs) if tag is None else self.loss_fn(bk.inputs, tag)
+            opt_kwargs = self.optimizer_kwargs
+            to_backward = loss
+            if self.loss_scaler is not None:
+                # the scale is a device scalar read by the graph: every micro-batch of an accumulation
+                # window carries the same scale, which moves only at the optimizer step (apex delay_unscale)
+                lid = self._loss_id(tag)
+                to_backward = self.loss_scaler.scale(loss, lid)
+                opt_kwargs = dict(opt_kwargs, grad_scale=self.loss_scaler, loss_id=lid)
             if self.reducer is not None:
-                self.reducer.backward_and_reduce(loss)
+                self.reducer.backward_and_reduce(to_backward)
             else:
-                loss.backward()
+                to_backward.backward()
             self.arena.finish_step()          # parameters this step never touched: exactly zero
-            if self.optimizer is not None:
-                self.optimizer.step(**self.optimizer_kwargs)
+            if self.optimizer is not None and step_optimizer:
+                self.optimizer.step(**opt_kwargs)
         finally:
             _model._RNG_GRAPH["dev"] = None
             self.arena.end_step_mode()
         return loss.detach()
 
-    def _capture(self, key, host_batch, lens, T_pad, maxseq, accumulate, tag=None):
+    def _capture(self, key, host_batch, lens, T_pad, maxseq, accumulate, tag=None, step_optimizer=True):
         bk = _Bucket()
         bk.T_pad, bk.maxseq, bk.n_replays = T_pad, maxseq, 0
         dev = self.device
@@ -155,7 +182,7 @@ class GraphedStep(object):
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
             for _ in range(self.warmup):
-                self._run(bk, accumulate, tag)
+                self._run(bk, accumulate, tag, step_optimizer)
             if saved is not None:
                 self.arena.flat.copy_(saved)
         torch.cuda.current_stream().wait_stream(s)
@@ -172,11 +199,11 @@ class GraphedStep(object):
         lib.ub200_launch_count.restype = __import__("ctypes").c_ulonglong
         n0 = lib.ub200_launch_count()
         if self.reducer_mode == "split":
-            self._capture_split(bk, accumulate, tag)
+            self._capture_split(bk, accumulate, tag, step_optimizer)
         else:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g, pool=self.pool, stream=self._cap_stream):
-                bk.loss = self._run(bk, accumulate, tag)
+                bk.loss = self._run(bk, accumulate, tag, step_optimizer)
             bk.graphs, bk.ship_after = [g], [[]]
         bk.launches = int(lib.ub200_launch_count() - n0)     # libub200 kernels inside one replay
         bk.graph = bk.graphs[0]
@@ -184,7 +211,7 @@ class GraphedStep(object):
         self.captures += 1
         return bk
 
-    def _capture_split(self, bk, accumulate, tag):
+    def _capture_split(self, bk, accumulate, tag, step_optimizer=True):
         """Capture the step as a chain of graphs, cut wherever the reducer reports that ranges of the
         arena are final (reducer._split_cb).  No NCCL call happens during the capture; on replay the
         ranges recorded for a cut are all-reduced right after the graph that ends there."""
@@ -213,7 +240,7 @@ class GraphedStep(object):
             try:
                 # the cuts end / begin captures from inside autograd's backward: keep it on this thread
                 with torch.autograd.set_multithreading_enabled(False):
-                    bk.loss = self._run(bk, accumulate, tag)
+                    bk.loss = self._run(bk, accumulate, tag, step_optimizer)
             finally:
                 self.reducer._split_cb = None
                 state["g"].capture_end()
@@ -241,15 +268,17 @@ class GraphedStep(object):
         return bk.loss
 
     # ------------------------------------------------------------------ public
-    def stage(self, host_batch, lens, accumulate=False, tag=None):
+    def stage(self, host_batch, lens, accumulate=False, tag=None, step_optimizer=True):
         """Copy a batch (pinned host tensors, or device tensors prefetched on a copy stream) into its
         bucket's static inputs (async, current stream) and return the bucket; capture the bucket's
         graph first if it is new.  `tag` (e.g. the pre-training task) becomes part of the bucket key and
-        is passed to loss_fn(batch, tag)."""
-        key, T_pad, maxseq = self._key(host_batch, lens, accumulate, tag)
+        is passed to loss_fn(batch, tag).  step_optimizer=False: the step ends after the backward (the
+        micro-batches of an accumulation window before its last one); it has its own graph."""
+        key, T_pad, maxseq = self._key(host_batch, lens, accumulate, tag, step_optimizer)
         bk = self.buckets.get(key)
         if bk is None:
-            bk = self._capture(key, host_batch, lens, T_pad, maxseq, accumulate, tag)
+            bk = self._capture(key, host_batch, lens, T_pad, maxseq, accumulate, tag,
+                               self._steps_optimizer(step_optimizer))
         for k, v in host_batch.items():
             if torch.is_tensor(v):
                 bk.inputs[k].copy_(v, non_blocking=True)
@@ -257,5 +286,5 @@ class GraphedStep(object):
         self._fill_meta(bk, lens, mask.size(1))
         return bk
 
-    def __call__(self, batch, lens, accumulate=False, tag=None):
-        return self.replay(self.stage(batch, lens, accumulate, tag))
+    def __call__(self, batch, lens, accumulate=False, tag=None, step_optimizer=True):
+        return self.replay(self.stage(batch, lens, accumulate, tag, step_optimizer))

@@ -44,6 +44,76 @@ def build_optimizer(model, opts):
     return FusedAdamW(groups, lr=opts.learning_rate, betas=tuple(opts.betas))
 
 
+def scaler_table(entries):
+    """Host image of a ub200_loss_scaler table: one (scale, unskipped, window, max_scale, min_scale)
+    tuple per loss id -> float32 [n, 8] (the int32 fields are stored bit-cast, read them through
+    .view(torch.int32)).  inv_scale starts at 1 / scale."""
+    arr = (_lib.LossScalerEntry * len(entries))()
+    for e, (scale, unskipped, window, max_scale, min_scale) in zip(arr, entries):
+        e.scale, e.unskipped, e.inv_scale = scale, unskipped, 1.0 / scale
+        e.window, e.max_scale, e.min_scale = window, max_scale, min_scale or 0.0
+    raw = bytearray(C.string_at(C.addressof(arr), C.sizeof(arr)))
+    return torch.frombuffer(raw, dtype=torch.float32).view(len(entries), C.sizeof(_lib.LossScalerEntry) // 4)
+
+
+class DynamicLossScaler(object):
+    """apex amp's dynamic loss scaler (``LossScaler``, dynamic mode; train_vqa.py:152,189-199), one
+    entry per loss id like pre-training's ``num_losses=len(task2scaler)`` (pretrain.py:230-233), held
+    in DEVICE memory at a fixed address (``self.table``, the C ABI's ``ub200_loss_scaler`` array).
+
+    ``scale(loss, k)`` multiplies by the device scalar, ``FusedAdamW.step(grad_scale=scaler,
+    loss_id=k)`` unscales by it and moves it after the overflow check, all on the device: a step
+    never reads the scale on the host, so it can be captured in a CUDA graph and replayed while the
+    scale changes.  Policy (apex): an overflowed step is skipped and halves the scale (not below
+    `min_scale`, if given); after `scale_window` clean steps in a row the scale doubles, up to
+    `max_scale`."""
+
+    def __init__(self, num_losses=1, init_scale=2.**16, scale_window=2000, max_scale=2.**24, min_scale=None,
+                 device=None):
+        if num_losses < 1:
+            raise ValueError("DynamicLossScaler: num_losses must be >= 1")
+        if not init_scale > 0 or not max_scale > 0 or scale_window < 1:
+            raise ValueError("DynamicLossScaler: need init_scale > 0, max_scale > 0 and scale_window >= 1")
+        self.num_losses = int(num_losses)
+        self.policy = (int(scale_window), float(max_scale), None if not min_scale else float(min_scale))
+        host = scaler_table([(float(init_scale), 0) + self.policy] * self.num_losses)
+        self.table = host.to(device if device is not None else torch.device("cuda", torch.cuda.current_device()))
+        self._scales = [self.table[k, 0] for k in range(self.num_losses)]     # 0-d views, built once
+
+    def _check_id(self, loss_id):
+        if not 0 <= loss_id < self.num_losses:
+            raise IndexError("DynamicLossScaler: loss_id %d out of range [0, %d)" % (loss_id, self.num_losses))
+
+    def scale(self, loss, loss_id=0):
+        """loss * current scale of `loss_id`, in fp32, as a device op (no host read)."""
+        self._check_id(loss_id)
+        return loss.float() * self._scales[loss_id]
+
+    def loss_scale(self, loss_id=0):
+        """Current scale of `loss_id` (host read: synchronises; for logging)."""
+        self._check_id(loss_id)
+        return float(self.table[loss_id, 0].item())
+
+    def unskipped(self, loss_id=0):
+        self._check_id(loss_id)
+        return int(self.table.view(torch.int32)[loss_id, 1].item())
+
+    def state_dict(self):
+        """What apex's ``amp.state_dict()`` stores: {'loss_scaler<k>': {'loss_scale', 'unskipped'}}."""
+        rows = self.table.cpu()
+        ints = rows.view(torch.int32)
+        return {"loss_scaler%d" % k: {"loss_scale": float(rows[k, 0]), "unskipped": int(ints[k, 1])}
+                for k in range(self.num_losses)}
+
+    def load_state_dict(self, sd):
+        if len(sd) != self.num_losses:
+            raise ValueError("DynamicLossScaler: state_dict has %d loss scalers, this one %d"
+                             % (len(sd), self.num_losses))
+        entries = [(float(sd["loss_scaler%d" % k]["loss_scale"]), int(sd["loss_scaler%d" % k]["unskipped"]))
+                   + self.policy for k in range(self.num_losses)]
+        self.table.copy_(scaler_table(entries))        # in place: the table keeps its address
+
+
 class FusedAdamW(object):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0,
                  correct_bias=True):
@@ -262,16 +332,20 @@ class FusedAdamW(object):
 
     # ------------------------------------------------------------------ step
     @torch.no_grad()
-    def step(self, grad_scale=1.0, max_grad_norm=-1.0):
+    def step(self, grad_scale=1.0, max_grad_norm=-1.0, loss_id=0):
         """One optimizer step over every parameter that has a gradient: global gradient norm
         (always — it is also the overflow detector), device-side bookkeeping, fused update.
 
-        grad_scale: the loss scale the gradients carry (they are multiplied by 1 / grad_scale);
+        grad_scale: the loss scale the gradients carry (they are multiplied by 1 / grad_scale), or a
+        DynamicLossScaler whose entry `loss_id` scaled the loss: the unscale factor is then read from
+        device memory and the scaler is updated on the device after the overflow check;
         max_grad_norm > 0: clip the global norm of the unscaled gradients like ``clip_grad_norm_``
         (the norm itself stays on the device: ``self.last_sumsq``).  A non-finite norm (fp16
         overflow) SKIPS the step on the device — masters, moments, weights and the step count stay
         untouched and ``self.found_inf`` is set — like apex's dynamic loss scaler does."""
         lib = _lib.load()
+        if isinstance(grad_scale, DynamicLossScaler):
+            return self._step_scaled(lib, grad_scale, int(loss_id), max_grad_norm)
         key = self._table_key()
         T = self._tables
         if T is None or T["key"] != key:
@@ -290,4 +364,31 @@ class FusedAdamW(object):
                                         T["betas"][0], T["betas"][1], T["eps"], 1.0 / float(grad_scale),
                                         float(max_grad_norm) if clip else -1.0, self.last_sumsq.data_ptr(),
                                         self._dev_state.data_ptr(), self._lr_dev.data_ptr(), stream))
+        return None
+
+    def _step_scaled(self, lib, scaler, loss_id, max_grad_norm):
+        scaler._check_id(loss_id)
+        key = self._table_key()
+        T = self._tables
+        if T is None or T["key"] != key:
+            T = self._build_tables(key)
+            if T is None:
+                return None
+        if scaler.table.device != self._dev_state.device:
+            raise RuntimeError("FusedAdamW: the loss scaler lives on %s, the parameters on %s"
+                               % (scaler.table.device, self._dev_state.device))
+        if not torch.cuda.is_current_stream_capturing():
+            self.sync_lr()
+        stream = _lib.current_stream()
+        self.last_sumsq.zero_()
+        _lib.check(lib.ub200_grad_sumsq(T["segs"].data_ptr(), T["starts"].data_ptr(), T["nseg"], T["nblocks"],
+                                        self.last_sumsq.data_ptr(), stream))
+        _lib.check(lib.ub200_adam_prep_scaled(self.last_sumsq.data_ptr(), self._dev_state.data_ptr(),
+                                              scaler.table.data_ptr(), loss_id, stream))
+        clip = max_grad_norm is not None and max_grad_norm > 0
+        _lib.check(lib.ub200_adamw_step_scaled(T["segs"].data_ptr(), T["starts"].data_ptr(), T["nseg"],
+                                               T["nblocks"], T["betas"][0], T["betas"][1], T["eps"],
+                                               float(max_grad_norm) if clip else -1.0, self.last_sumsq.data_ptr(),
+                                               self._dev_state.data_ptr(), self._lr_dev.data_ptr(),
+                                               scaler.table.data_ptr(), loss_id, stream))
         return None
