@@ -54,6 +54,27 @@ unsigned long long ub200_launch_count(void);  /* kernels launched by this librar
  * device); returns the previous value.  Used by uniter_b200.distributed.GradientReducer while the
  * chunked all-reduce overlaps the backward pass (replaces utils/distributed.py:16-43). */
 int ub200_set_sm_reserve(int n);
+/* Deterministic mode (on != 0; returns the previous value).  Read at launch time, like the SM reserve,
+ * so a captured CUDA graph keeps the mode it was captured under.  With the mode on, the reductions
+ * below use no floating-point atomics and no summation order that depends on the grid (so neither the
+ * SM reserve nor appended all-zero padding rows change their bits).  A whole training step is not yet
+ * bit-reproducible in this mode (see DESIGN.md section 3b).  The forms it selects:
+ *   column sums (ub200_colsum, UB200_EPI_COLSUM, the attention's dbias, the LayerNorm backward's
+ *     dgamma / dbeta / dbias, ub200_embed_bwd_colsums): one CTA owns 8 columns, thread t sums rows
+ *     t, t + 256, ... in ascending order, the 256 partials meet in a fixed tree;
+ *   UB200_EPI_COLSUM sums the 16-bit output after the GEMM instead of the fp32 values in its epilogue;
+ *   k_splits / UB200_EPI_ATOMIC: no split-K, each element is summed over all of K by one CTA;
+ *   ub200_layernorm_bwd: always the split form, so stats_ws is REQUIRED (rows x 2 floats), for the
+ *     row_kind / dropout_on_dy cases too;
+ *   ub200_embed_bwd_scatter: each table row is owned by the first packed row with that id, which sums
+ *     all its rows in ascending order in fp32 and adds to the table once (hidden <= 1024);
+ *   ub200_grad_sumsq is an error: use ub200_grad_sumsq_ws (one partial per ub200_adam_chunk() block,
+ *     summed in block order);
+ *   ub200_attn_bwd: max_seqlen <= 128 only (UB200_EUNSUPPORTED otherwise);
+ *   the GEMM tile shape is chosen for 132 SMs whatever the reserve.
+ * Nothing changes with the mode off. */
+int ub200_set_deterministic(int on);
+int ub200_deterministic(void);            /* the current value */
 int ub200_profile_enable(int on);
 int ub200_profile_collect(float* ms_per_tag, int* launches_per_tag, int ntags);
 
@@ -438,6 +459,13 @@ enum { UB200_F32 = 2 };
 int32_t ub200_adam_chunk(void);
 int ub200_grad_sumsq(const ub200_adam_segment* segs_dev, const int32_t* blk_start_dev, int32_t nseg,
                      int32_t nblocks, float* out, ub200_stream_t stream);
+/* ub200_grad_sumsq with caller-owned scratch of ub200_grad_sumsq_workspace_bytes(nblocks) bytes (4-byte
+ * aligned), which the deterministic mode needs (a smaller one is UB200_EINVAL); with the mode off the
+ * workspace is not touched. */
+int64_t ub200_grad_sumsq_workspace_bytes(int32_t nblocks);
+int ub200_grad_sumsq_ws(const ub200_adam_segment* segs_dev, const int32_t* blk_start_dev, int32_t nseg,
+                        int32_t nblocks, float* out, void* workspace, int64_t workspace_bytes,
+                        ub200_stream_t stream);
 /* state_dev / lr_dev NULL: legacy mode (host-computed step_size / lr_wd per segment, no skipping).
  * Otherwise: skip when state->found_inf; lr = lr_dev[seg.group]; bias correction from state->step. */
 int ub200_adamw_step(const ub200_adam_segment* segs_dev, const int32_t* blk_start_dev, int32_t nseg,

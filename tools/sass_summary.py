@@ -1,5 +1,6 @@
 """Per-kernel SASS mnemonic counts of libub200.so (cuobjdump -sass): which kernels are wgmma (HGMMA) / TMA,
-and — for the peer exchange — which carry system-scope release / acquire accesses.
+which — for the peer exchange — carry system-scope release / acquire accesses, and which carry
+floating-point RED / ATOM instructions (order-dependent sums: none in the deterministic mode's kernels).
 
     python tools/sass_summary.py > sass_summary.txt
 """
@@ -15,7 +16,10 @@ COLS = [("HGMMA", r"\bHGMMA"), ("UTMALDG", r"\bUTMALDG"), ("UTMASTG", r"\bUTMAST
         ("WARPGROUP", r"\bWARPGROUP"),
         ("MUFU.EX2", r"MUFU\.EX2"), ("MUFU.RCP", r"MUFU\.RCP"), ("MUFU.TANH", r"MUFU\.TANH"),
         ("STG.SYS", r"\bSTG\.E(\.\w+)*\.STRONG\.SYS"), ("LDG.SYS", r"\bLDG\.E(\.\w+)*\.STRONG\.SYS"),
-        ("MEMBAR.SYS", r"MEMBAR\.\w+\.SYS")]
+        ("MEMBAR.SYS", r"MEMBAR\.\w+\.SYS"),
+        # floating-point reductions / atomics to memory: their order depends on scheduling, so a kernel
+        # the deterministic mode launches must have none (integer tickets are fine)
+        ("FP.RED/ATOM", r"\b(RED|REDG|ATOM|ATOMG)\.[\w.]*\b(F16x2|BF16x2|F32|F32x\d|F64)\b")]
 
 
 def main():

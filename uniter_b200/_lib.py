@@ -133,6 +133,10 @@ def load():
     lib.ub200_device_check.restype = C.c_int
     lib.ub200_set_sm_reserve.restype = C.c_int
     lib.ub200_set_sm_reserve.argtypes = [C.c_int]
+    lib.ub200_set_deterministic.restype = C.c_int
+    lib.ub200_set_deterministic.argtypes = [C.c_int]
+    lib.ub200_deterministic.restype = C.c_int
+    lib.ub200_deterministic.argtypes = []
     lib.ub200_gemm.restype = C.c_int
     lib.ub200_gemm.argtypes = [C.POINTER(GemmArgs), C.c_void_p]
     lib.ub200_gemm_grouped.restype = C.c_int
@@ -180,6 +184,11 @@ def load():
     lib.ub200_adam_chunk.restype = C.c_int32
     lib.ub200_grad_sumsq.restype = C.c_int
     lib.ub200_grad_sumsq.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
+    lib.ub200_grad_sumsq_workspace_bytes.restype = C.c_int64
+    lib.ub200_grad_sumsq_workspace_bytes.argtypes = [C.c_int32]
+    lib.ub200_grad_sumsq_ws.restype = C.c_int
+    lib.ub200_grad_sumsq_ws.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                        C.c_int64, C.c_void_p]
     lib.ub200_adamw_step.restype = C.c_int
     lib.ub200_adamw_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_float,
                                      C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -227,6 +236,11 @@ def dtype_code(t, allow_f32=False):
 
 def ptr(t):
     return None if t is None else t.data_ptr()
+
+
+def deterministic():
+    """Whether the library's deterministic mode (ub200_set_deterministic) is on: read from the library."""
+    return bool(load().ub200_deterministic())
 
 
 def current_stream():

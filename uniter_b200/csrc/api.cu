@@ -40,6 +40,10 @@ int set_sm_reserve(int n) {
   return prev;
 }
 
+static int g_deterministic = 0;
+
+int deterministic() { return g_deterministic; }
+
 static PFN_cuTensorMapEncodeTiled_v12000 get_encode() {
   static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
   if (fn == nullptr) {
@@ -147,6 +151,14 @@ extern "C" {
 unsigned long long ub200_launch_count(void) { return ub::g_launches; }
 
 int ub200_set_sm_reserve(int n) { return ub::set_sm_reserve(n); }
+
+int ub200_set_deterministic(int on) {
+  const int prev = ub::g_deterministic;
+  ub::g_deterministic = on ? 1 : 0;
+  return prev;
+}
+
+int ub200_deterministic(void) { return ub::g_deterministic; }
 
 int ub200_profile_enable(int on) {
   ub::g_prof_on = on != 0;

@@ -439,7 +439,9 @@ __device__ __forceinline__ void dq_block(float (&dq)[32], uint32_t uDS, uint32_t
   wgmma_wait<0>();
 }
 
-template <bool kBF16>
+// kBias = false: the deterministic mode's instantiation, with no bias-gradient flush (its float atomics);
+// that mode sums the bias gradient from dqkv with launch_colsum_det instead.
+template <bool kBF16, bool kBias = true>
 __global__ void __launch_bounds__(SH_THREADS, 2)
 attn_bwd_short_kernel(const __grid_constant__ CUtensorMap tmQKV64, const __grid_constant__ CUtensorMap tmDO64,
                       const AttnParams p) {
@@ -594,7 +596,7 @@ attn_bwd_short_kernel(const __grid_constant__ CUtensorMap tmQKV64, const __grid_
         key[e] = 64 * kb + r_loc[e];
         k_ok[e] = key[e] < S;
       }
-      if (p.dbias) {   // key / value bias gradients
+      if (kBias && p.dbias) {   // key / value bias gradients
         frag_colsum64_warp(dk, k_ok[0], k_ok[1], sBias[warp] + ATT_D, lane);
         frag_colsum64_warp(dv, k_ok[0], k_ok[1], sBias[warp] + 2 * ATT_D, lane);
       }
@@ -615,7 +617,7 @@ attn_bwd_short_kernel(const __grid_constant__ CUtensorMap tmQKV64, const __grid_
       bool q_ok[2];
 #pragma unroll
       for (int e = 0; e < 2; ++e) q_ok[e] = 64 * qb + r_loc[e] < S;
-      if (p.dbias) frag_colsum64_warp(dq, q_ok[0], q_ok[1], sBias[warp], lane);   // query-bias gradient
+      if (kBias && p.dbias) frag_colsum64_warp(dq, q_ok[0], q_ok[1], sBias[warp], lane);   // query-bias gradient
 #pragma unroll
       for (int e = 0; e < 2; ++e)
         if (q_ok[e])
@@ -625,7 +627,7 @@ attn_bwd_short_kernel(const __grid_constant__ CUtensorMap tmQKV64, const __grid_
     }
     wg_sync();   // every wgmma reading this stage, sP and sDS has completed; sBias is complete
     if (nx.valid() && !pre && tid == 0) load(nx, 0);
-    if (p.dbias && (!nx.valid() || nx.h != head)) {
+    if (kBias && p.dbias && (!nx.valid() || nx.h != head)) {
       // one atomic per column and head change: this CTA's share of the bias gradient of `head`
       for (int i = tid; i < 3 * ATT_D; i += SH_THREADS) {
         atomicAdd(p.dbias + (i >> 6) * p.H + head * ATT_D + (i & 63),
@@ -1122,6 +1124,36 @@ extern "C" int ub200_attn_bwd(const ub200_attn_args* args, ub200_stream_t stream
   AttnParams p = attn_params(a);
   p.dctx = a.dctx; p.dqkv = a.dqkv; p.dbias = a.dbias;
   const int di = a.dtype == UB200_BF16 ? 1 : 0;
+
+  if (deterministic()) {
+    // dQ of a sequence longer than one key block is summed over key blocks with float atomics; no
+    // fixed-order form of the long kernels exists yet
+    if (a.max_seqlen > SH_MAXSEQ)
+      return set_error(UB200_EUNSUPPORTED, "attn_bwd: deterministic mode supports max_seqlen <= %d (got %d)",
+                       SH_MAXSEQ, a.max_seqlen);
+    CUtensorMap tmQ, tmD;
+    int rc = make_tma_2d(&tmQ, a.qkv, a.dtype, a.total_tokens, 3 * a.hidden, 3 * a.hidden, 64, ATT_D);
+    if (rc) return rc;
+    rc = make_tma_2d(&tmD, a.dctx, a.dtype, a.total_tokens, a.hidden, a.hidden, 64, ATT_D);
+    if (rc) return rc;
+    p.dbias = nullptr;
+    void (*kern)(const CUtensorMap, const CUtensorMap, const AttnParams) =
+        di ? attn_bwd_short_kernel<true, false> : attn_bwd_short_kernel<false, false>;
+    static unsigned long long configured[2] = {0, 0};   // one bit per device
+    if (first_use_on_device(configured[di]))
+      UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SH_BWD_SMEM));
+    {
+      ProfScope ps(stream);
+      UB_CHECK_CUDA(launch_pdl(kern, short_grid(a, 2), dim3(SH_THREADS), SH_BWD_SMEM, stream, 1, tmQ, tmD, p));
+    }
+    UB_CHECK_CUDA(cudaGetLastError());
+    // QKV bias gradient: fixed-order column sums of the 16-bit dqkv, over the rows of the sequences only
+    // (rows past cu_seqlens[batch] are not written by the kernel)
+    if (a.dbias)
+      return launch_colsum_det(a.dtype, a.dqkv, a.dbias, a.total_tokens, 3 * a.hidden, 3 * a.hidden, stream,
+                               a.cu_seqlens + a.batch);
+    return 0;
+  }
 
   if (a.max_seqlen <= SH_MAXSEQ) {
     CUtensorMap tmQ, tmD;

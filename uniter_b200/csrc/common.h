@@ -24,6 +24,13 @@ int set_error(int code, const char* fmt, ...);  // stores message, returns code
   } while (0)
 
 int num_sms();  // SM count of the current device (cached)
+int deterministic();  // ub200_set_deterministic: launches use fixed-order reductions, no float atomics
+
+// out[n] += sum_m x[m, n] in a fixed order (rows m ≡ lane mod 256, then a fixed tree): the bits depend
+// on the values and their row indices only, and appended zero rows leave them unchanged.
+// rows_dev (optional, device): only rows < min(rows, *rows_dev) are summed (e.g. &cu_seqlens[batch]).
+int launch_colsum_det(int dtype, const void* x, float* out, int rows, int N, long long ld,
+                      cudaStream_t stream, const int* rows_dev = nullptr);
 
 // cudaFuncSetAttribute is per DEVICE: one bit per device in a per-instantiation mask (a process that
 // drives several GPUs configures each of them once).  Returns true the first time for this device.

@@ -331,6 +331,69 @@ embed_bwd_scatter_kernel(const void* __restrict__ du_, const int* __restrict__ k
   }
 }
 
+// Deterministic form (one CTA of 128 threads per packed row; blockIdx.y = 0 word table, 1 position
+// table).  The CTA of the FIRST text row with a given id owns that id: it sums the du rows of every
+// text row with the id in ascending row order in fp32 (8 columns per thread) and adds the total to the
+// table row once, rounding once as torch's deterministic embedding backward does.  Other rows exit
+// after the ownership scan.  Needs hidden <= 1024.
+template <bool kBF16>
+__global__ void __launch_bounds__(128)
+embed_bwd_scatter_det_kernel(const void* __restrict__ du_, const int* __restrict__ kind,
+                             const int* __restrict__ word_id, const int* __restrict__ pos_id,
+                             void* __restrict__ d_word_, float* __restrict__ d_pos, int T, int H) {
+  pdl_launch_dependents();
+  pdl_wait();
+  using T16 = typename Elem<kBF16>::T;
+  __shared__ unsigned match[4];
+  const int t = blockIdx.x;
+  if (kind[t] != 0) return;
+  const int* ids = blockIdx.y ? pos_id : word_id;
+  const int id = ids[t];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  bool earlier = false;
+  for (int r = tid; r < t && !earlier; r += 128) earlier = kind[r] == 0 && ids[r] == id;
+  if (__syncthreads_or(earlier)) return;
+  const int v = tid;                         // this thread's 8 columns
+  const bool col_ok = v < (H >> 3);
+  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int base = t; base < T; base += 128) {
+    const int r = base + tid;
+    const bool m = r < T && kind[r] == 0 && ids[r] == id;
+    const unsigned b = __ballot_sync(0xffffffffu, m);
+    if (lane == 0) match[warp] = b;
+    __syncthreads();
+    if (col_ok) {
+      for (int w = 0; w < 4; ++w) {
+        unsigned bits = match[w];
+        while (bits) {
+          const int row = base + w * 32 + __ffs(bits) - 1;
+          bits &= bits - 1;
+          float f[8];
+          e_unpack8<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(du_) +
+                                                                static_cast<size_t>(row) * H) + v), f);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) acc[e] += f[e];
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (!col_ok) return;
+  if (blockIdx.y == 0) {
+    uint4* w = reinterpret_cast<uint4*>(reinterpret_cast<T16*>(d_word_) + static_cast<size_t>(id) * H) + v;
+    float cur[8];
+    e_unpack8<kBF16>(*w, cur);
+    uint32_t o[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) o[q] = Elem<kBF16>::pack(cur[2 * q] + acc[2 * q], cur[2 * q + 1] + acc[2 * q + 1]);
+    *w = make_uint4(o[0], o[1], o[2], o[3]);
+  } else {
+    float* prow = d_pos + static_cast<size_t>(id) * H + v * 8;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) prow[e] += acc[e];
+  }
+}
+
 // ------------------------------------------------------------------------------ weighted column sums
 //   out[k * stride_k + n * stride_n] += sum_t w_k(t) * x[t, n],   k < W
 // mode 0  w_k(t) = (type_id[t] - base == k)               -> token_type table gradient [Ty, H]
@@ -413,6 +476,53 @@ wcolsum_kernel(const WColsumParams p) {
       for (int w8 = 0; w8 < 8; ++w8) s += red[w8][c];
       if (s != 0.f) atomicAdd(p.out + k * p.stride_k + col * p.stride_n, s);
     }
+  }
+}
+
+// Deterministic form: CTA = 8 columns x 256 row lanes over all rows (det_tree_sum8), one owner per output.
+template <bool kBF16>
+__global__ void __launch_bounds__(256)
+wcolsum_det_kernel(const WColsumParams p) {
+  pdl_launch_dependents();
+  pdl_wait();
+  using T16 = typename Elem<kBF16>::T;
+  constexpr int W = 8;
+  __shared__ float red[256][9];
+  const int col0 = blockIdx.x * 8;
+  float acc[W][8];
+#pragma unroll
+  for (int k = 0; k < W; ++k)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[k][e] = 0.f;
+  for (int r = threadIdx.x; r < p.T; r += 256) {
+    float w[W];
+#pragma unroll
+    for (int k = 0; k < W; ++k) w[k] = 0.f;
+    if (p.mode == 0) {
+      const int ty = p.type_id[r] - p.base;
+      if (ty < 0 || ty >= W) continue;
+#pragma unroll
+      for (int k = 0; k < W; ++k) w[k] = (ty == k) ? 1.f : 0.f;
+    } else {
+      const int s = p.img_src[r];
+      if (p.kind[r] != 1 || s < 0) continue;
+      const float* box = p.pos_feat + static_cast<size_t>(s) * 7;
+#pragma unroll
+      for (int k = 0; k < 7; ++k) w[k] = Elem<kBF16>::to_f(Elem<kBF16>::from_f(__ldg(box + k)));
+    }
+    float f[8];
+    e_unpack8<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.x) +
+                                                          static_cast<size_t>(r) * p.N + col0)), f);
+#pragma unroll
+    for (int k = 0; k < W; ++k)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[k][e] = fmaf(w[k], f[e], acc[k][e]);
+  }
+#pragma unroll
+  for (int k = 0; k < W; ++k) {
+    if (k >= p.nweights) break;     // uniform
+    const float s = det_tree_sum8(acc[k], red);
+    if (threadIdx.x < 8) p.out[k * p.stride_k + (col0 + threadIdx.x) * p.stride_n] += s;
   }
 }
 
@@ -524,6 +634,17 @@ extern "C" int ub200_embed_bwd_scatter(const void* du, const int32_t* kind, cons
   UB_CHECK_ARG(du && kind && word_id && pos_id && d_word && d_pos, "embed_bwd_scatter: null pointer");
   UB_CHECK_ARG(T > 0 && hidden > 0 && hidden % 8 == 0, "embed_bwd_scatter: need T > 0, hidden %% 8 == 0");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (deterministic()) {
+    UB_CHECK_ARG(hidden <= 1024, "embed_bwd_scatter: deterministic mode needs hidden <= 1024");
+    ProfScope ps(stream);
+    if (dtype == UB200_BF16)
+      UB_CHECK_CUDA(launch_pdl(embed_bwd_scatter_det_kernel<true>, dim3(T, 2), dim3(128), 0, stream, 1, du, kind,
+                               word_id, pos_id, d_word, d_pos, T, hidden));
+    else
+      UB_CHECK_CUDA(launch_pdl(embed_bwd_scatter_det_kernel<false>, dim3(T, 2), dim3(128), 0, stream, 1, du, kind,
+                               word_id, pos_id, d_word, d_pos, T, hidden));
+    return 0;
+  }
   const int grid = (T + 7) / 8;
   ProfScope ps(stream);
   if (dtype == UB200_BF16)
@@ -558,6 +679,13 @@ extern "C" int ub200_embed_bwd_colsums(const ub200_embed_colsum_args* a, ub200_s
     if (a->mode == 0) { p.stride_k = a->hidden; p.stride_n = 1; p.out = a->out + static_cast<long long>(base) * a->hidden; }
     else { p.stride_k = 1; p.stride_n = 7; }
     ProfScope ps(stream);
+    if (deterministic()) {
+      if (a->dtype == UB200_BF16)
+        UB_CHECK_CUDA(launch_pdl(wcolsum_det_kernel<true>, dim3(a->hidden / 8), dim3(256), 0, stream, 1, p));
+      else
+        UB_CHECK_CUDA(launch_pdl(wcolsum_det_kernel<false>, dim3(a->hidden / 8), dim3(256), 0, stream, 1, p));
+      continue;
+    }
     if (a->dtype == UB200_BF16)
       UB_CHECK_CUDA(launch_pdl(wcolsum_kernel<true>, dim3(gx, gy), dim3(256), 0, stream, 1, p));
     else

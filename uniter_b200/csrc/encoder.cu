@@ -238,7 +238,7 @@ extern "C" int ub200_encoder_bwd(const ub200_encoder_desc* d, const ub200_layer_
   const int acc = accumulate_wgrad ? UB200_EPI_ACCUM : 0;
   // UB200_LN_BWD_SPLIT=1: row kernel + column kernel instead of the fused LayerNorm backward (A/B runs)
   static const bool ln_split = [] { const char* e = getenv("UB200_LN_BWD_SPLIT"); return e && e[0] == '1'; }();
-  float* ln_ws = ln_split ? reinterpret_cast<float*>(sc + S.ln_stats) : nullptr;
+  float* ln_ws = (ln_split || deterministic()) ? reinterpret_cast<float*>(sc + S.ln_stats) : nullptr;
 
   const void* dcur = d_layer_out[NL - 1];
   int pp = 0;  // ping-pong for the running gradient

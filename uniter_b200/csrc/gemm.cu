@@ -39,6 +39,10 @@ static void pick_config(int M, int N, int K, int sms, int* bn_out, int* cluster_
   }
 }
 
+// SM count the tile heuristics assume in the deterministic mode (that of an H100 SXM), so that the tile
+// shape, and with it every output bit, cannot change with ub200_set_sm_reserve.
+constexpr int DET_CONFIG_SMS = 132;
+
 }  // namespace ub
 
 extern "C" int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream_) {
@@ -70,6 +74,22 @@ extern "C" int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream_) {
                "gemm: k_splits > 1 needs EPI_ATOMIC | EPI_OUT_F32 and a zeroed output");
   UB_CHECK_ARG(a.n_valid >= 0 && a.n_valid <= a.N, "gemm: n_valid must be in [0, N]");
   const int n_valid = a.n_valid ? a.n_valid : a.N;
+
+  if (deterministic() && (epi & (UB200_EPI_COLSUM | UB200_EPI_ATOMIC))) {
+    // Fixed-order forms.  Split-K is not used: one CTA sums each output element over all of K and adds
+    // it to the (zeroed) output, so the split count can depend on nothing.  The bias gradient is a
+    // fixed-order column sum of the 16-bit output, as nn.Linear's bias gradient sums the 16-bit grad.
+    UB_CHECK_ARG(!((epi & UB200_EPI_COLSUM) && (epi & UB200_EPI_OUT_F32)),
+                 "gemm: EPI_COLSUM needs a 16-bit output in deterministic mode");
+    ub200_gemm_args b = a;
+    b.epilogue = epi & ~(UB200_EPI_COLSUM | UB200_EPI_ATOMIC);
+    if (epi & UB200_EPI_ATOMIC) b.epilogue |= UB200_EPI_ACCUM;
+    b.colsum = nullptr;
+    b.k_splits = 0;
+    const int rc = ub200_gemm(&b, stream_);
+    if (rc || !(epi & UB200_EPI_COLSUM)) return rc;
+    return launch_colsum_det(a.dtype, a.out, a.colsum, a.M, a.N, a.ldo, stream);
+  }
 
   if (epi & UB200_EPI_LN) {
     // fused residual + LayerNorm epilogue: its own kernel (4-CTA cluster over N), see gemm_ln.cu
@@ -115,7 +135,8 @@ extern "C" int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream_) {
 
   const int sms = num_sms();
   int bn = 0, cluster = 0;
-  pick_config(a.M, a.N, a.K, sms, &bn, &cluster);
+  // deterministic mode: the tile shape is a function of (M, N, K) only, never of the SM reserve
+  pick_config(a.M, a.N, a.K, deterministic() ? DET_CONFIG_SMS : sms, &bn, &cluster);
   if (a.tile_n) {
     bn = a.tile_n;
     if (!a.cluster) cluster = ((bn == 128 || bn == 256) && a.M > BM) ? 2 : 1;
@@ -218,7 +239,8 @@ extern "C" int ub200_gemm_grouped(const ub200_gemm_args* args, int32_t count, ub
     for (int c = 0; c < 3; ++c) {
       int t = 0;
       for (int i = 0; i < count; ++i) t += ((args[i].M + BM - 1) / BM) * ((args[i].N + cand[c] - 1) / cand[c]);
-      const double cost = static_cast<double>((t + sms - 1) / sms) * (421.0 + 1.27 * cand[c]);
+      const int cs = deterministic() ? DET_CONFIG_SMS : sms;   // tile shape independent of the SM reserve
+      const double cost = static_cast<double>((t + cs - 1) / cs) * (421.0 + 1.27 * cand[c]);
       if (cost < best - 1e-9) { best = cost; bn = cand[c]; }
     }
   }

@@ -87,7 +87,11 @@ template <int EPI, bool kBF16>
 struct EpiMask {
   const int rt;
   __device__ __forceinline__ explicit EpiMask(int runtime) : rt(runtime) {}
-  __device__ __forceinline__ bool has(int bit) const { return EPI >= 0 ? (EPI & bit) != 0 : (rt & bit) != 0; }
+  // EPI == -2: runtime mask of the deterministic mode, built without the atomic epilogues
+  __device__ __forceinline__ bool has(int bit) const {
+    if (EPI == -2 && (bit & (UB200_EPI_COLSUM | UB200_EPI_ATOMIC))) return false;
+    return EPI >= 0 ? (EPI & bit) != 0 : (rt & bit) != 0;
+  }
 };
 
 // The fragment scatters a row over 4 lanes in 2-column pieces; storing (or loading side inputs)
@@ -522,31 +526,37 @@ static int launch_gemm(const GemmParams& p, const CUtensorMap& tmA, const CUtens
 }
 
 // Epilogue masks the encoder uses get their own instantiation (per operand-major form); any
-// other mask runs the runtime-flag kernel (EPI = -1).
+// other mask runs the runtime-flag kernel (EPI = -1, or -2 in deterministic mode).
 template <int BN, bool kBF16, int kCluster>
 static int dispatch_major(int a_major, int b_major, const GemmParams& p, const CUtensorMap& tmA,
                           const CUtensorMap& tmB, int grid, cudaStream_t stream) {
   const int e = p.epilogue;
+  const bool det = deterministic();
 #define UB_CASE(AMN, BMN, MASK) \
   if (e == (MASK)) return launch_gemm<BN, AMN, BMN, kBF16, kCluster, (MASK)>(p, tmA, tmB, grid, stream)
+#define UB_GENERIC(AMN, BMN)                                                                      \
+  return det ? launch_gemm<BN, AMN, BMN, kBF16, kCluster, -2>(p, tmA, tmB, grid, stream)         \
+             : launch_gemm<BN, AMN, BMN, kBF16, kCluster, -1>(p, tmA, tmB, grid, stream)
   if (a_major == 0 && b_major == 0) {            // forward nn.Linear
     UB_CASE(false, false, UB200_EPI_BIAS);
     UB_CASE(false, false, UB200_EPI_BIAS | UB200_EPI_GELU);
     UB_CASE(false, false, UB200_EPI_BIAS | UB200_EPI_RESIDUAL);
     UB_CASE(false, false, UB200_EPI_BIAS | UB200_EPI_DROPOUT | UB200_EPI_RESIDUAL);
-    return launch_gemm<BN, false, false, kBF16, kCluster, -1>(p, tmA, tmB, grid, stream);
+    UB_GENERIC(false, false);
   }
   if (a_major == 0 && b_major == 1) {            // dgrad
     UB_CASE(false, true, 0);
     UB_CASE(false, true, UB200_EPI_RESIDUAL);
     UB_CASE(false, true, UB200_EPI_DGELU | UB200_EPI_COLSUM);
-    return launch_gemm<BN, false, true, kBF16, kCluster, -1>(p, tmA, tmB, grid, stream);
+    if (det) UB_CASE(false, true, UB200_EPI_DGELU);   // DGELU | COLSUM of the deterministic mode
+    UB_GENERIC(false, true);
   }
   if (a_major == 1 && b_major == 1) {            // wgrad
     UB_CASE(true, true, 0);
     UB_CASE(true, true, UB200_EPI_ACCUM);
-    return launch_gemm<BN, true, true, kBF16, kCluster, -1>(p, tmA, tmB, grid, stream);
+    UB_GENERIC(true, true);
   }
+#undef UB_GENERIC
 #undef UB_CASE
   return set_error(UB200_EUNSUPPORTED, "gemm: a_major=1 with b_major=0 is not instantiated");
 }

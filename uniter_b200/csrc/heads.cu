@@ -173,7 +173,9 @@ __device__ __forceinline__ float grad_of(const ub200_adam_segment& sg, long long
   return reinterpret_cast<const float*>(sg.grad)[i];
 }
 
-// sum of squares of all gradients (before unscaling) -> out[0] (fp32, atomically accumulated)
+// sum of squares of all gradients (before unscaling) -> out[0] (fp32, atomically accumulated);
+// kDet: each block's sum to out[blockIdx.x] instead
+template <bool kDet>
 __global__ void __launch_bounds__(256)
 sumsq_kernel(const ub200_adam_segment* __restrict__ segs, const int* __restrict__ blk_start, int nseg,
              float* __restrict__ out) {
@@ -205,7 +207,25 @@ sumsq_kernel(const ub200_adam_segment* __restrict__ segs, const int* __restrict_
     }
   }
   acc = block_sum(acc, red);
-  if (threadIdx.x == 0 && acc != 0.f) atomicAdd(out, acc);
+  if (kDet) {
+    if (threadIdx.x == 0) out[blockIdx.x] = acc;   // partials[block]; summed by sumsq_finish_kernel
+  } else if (threadIdx.x == 0 && acc != 0.f) {
+    atomicAdd(out, acc);
+  }
+}
+
+// Deterministic mode: out[0] += sum of partials[0 .. nblocks) in a fixed order (thread t sums blocks
+// t, t + 256, ... ascending, then det_tree_sum8) -- the blocks are ADAM_CHUNK slices of the
+// segments, so the result does not depend on the grid.
+__global__ void __launch_bounds__(256)
+sumsq_finish_kernel(const float* __restrict__ partials, int nblocks, float* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float red[256][9];
+  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int b = threadIdx.x; b < nblocks; b += 256) acc[0] += partials[b];
+  const float s = det_tree_sum8(acc, red);
+  if (threadIdx.x == 0) out[0] += s;
 }
 
 struct AdamHyper {
@@ -435,10 +455,38 @@ extern "C" int ub200_grad_sumsq(const ub200_adam_segment* segs_dev, const int32_
                                 int32_t nseg, int32_t nblocks, float* out, ub200_stream_t stream_) {
   using namespace ub;
   UB_CHECK_ARG(segs_dev && blk_start_dev && out && nseg > 0 && nblocks > 0, "grad_sumsq: bad argument");
+  UB_CHECK_ARG(!deterministic(), "grad_sumsq: deterministic mode needs ub200_grad_sumsq_ws");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ProfScope ps(stream);
-  UB_CHECK_CUDA(launch_pdl(sumsq_kernel, dim3(nblocks), dim3(256), 0, stream, 1, segs_dev, blk_start_dev,
+  UB_CHECK_CUDA(launch_pdl(sumsq_kernel<false>, dim3(nblocks), dim3(256), 0, stream, 1, segs_dev, blk_start_dev,
                            nseg, out));
+  return 0;
+}
+
+extern "C" int64_t ub200_grad_sumsq_workspace_bytes(int32_t nblocks) {
+  return nblocks > 0 ? static_cast<int64_t>(nblocks) * 4 : 0;
+}
+
+extern "C" int ub200_grad_sumsq_ws(const ub200_adam_segment* segs_dev, const int32_t* blk_start_dev,
+                                   int32_t nseg, int32_t nblocks, float* out, void* workspace,
+                                   int64_t workspace_bytes, ub200_stream_t stream_) {
+  using namespace ub;
+  if (!deterministic()) return ub200_grad_sumsq(segs_dev, blk_start_dev, nseg, nblocks, out, stream_);
+  UB_CHECK_ARG(segs_dev && blk_start_dev && out && nseg > 0 && nblocks > 0, "grad_sumsq: bad argument");
+  UB_CHECK_ARG(workspace && (reinterpret_cast<uintptr_t>(workspace) & 3) == 0, "grad_sumsq: bad workspace");
+  UB_CHECK_ARG(workspace_bytes >= ub200_grad_sumsq_workspace_bytes(nblocks),
+               "grad_sumsq: workspace of %lld bytes, %lld needed", (long long)workspace_bytes,
+               (long long)ub200_grad_sumsq_workspace_bytes(nblocks));
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  float* partials = reinterpret_cast<float*>(workspace);
+  {
+    ProfScope ps(stream);
+    UB_CHECK_CUDA(launch_pdl(sumsq_kernel<true>, dim3(nblocks), dim3(256), 0, stream, 1, segs_dev, blk_start_dev,
+                             nseg, partials));
+  }
+  ProfScope ps(stream);
+  UB_CHECK_CUDA(launch_pdl(sumsq_finish_kernel, dim3(1), dim3(256), 0, stream, 1,
+                           static_cast<const float*>(partials), nblocks, out));
   return 0;
 }
 

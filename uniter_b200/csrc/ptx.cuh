@@ -226,6 +226,28 @@ __device__ __forceinline__ uint32_t rand16_of(const uint4& r, int lane8) {
   return (lane8 & 1) ? (w >> 16) : (w & 0xFFFFu);
 }
 
+// ---------------------------------------------------------------- fixed-order column reduction
+// Deterministic mode: a 256-thread CTA owns 8 columns; thread t has summed rows t, t + 256, ... in
+// ascending order into v[8].  The 256 partials meet in a fixed binary tree, so the result is a
+// function of the values and their row indices only (never of the grid).  Returns the total of
+// column e in thread e (e < 8).  `red` is 256 x 9 floats of shared memory.
+__device__ __forceinline__ float det_tree_sum8(const float (&v)[8], float (*red)[9]) {
+  const int t = threadIdx.x;
+  __syncthreads();                       // `red` may still be read by a previous call
+#pragma unroll
+  for (int e = 0; e < 8; ++e) red[t][e] = v[e];
+  __syncthreads();
+#pragma unroll
+  for (int s = 128; s > 0; s >>= 1) {
+    if (t < s) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) red[t][e] += red[t + s][e];
+    }
+    __syncthreads();
+  }
+  return t < 8 ? red[0][t] : 0.f;
+}
+
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

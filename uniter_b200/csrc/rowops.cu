@@ -310,6 +310,17 @@ ln_bwd_rows_kernel(const LnBwdParams p, float2* __restrict__ stats) {
   if (row >= p.rows) return;
   const int H = p.H, nvec = H >> 3;
   const float inv_h = 1.0f / H;
+  if (p.row_kind != nullptr && p.row_kind[row] != p.kind) {   // deterministic mode only
+    if (p.zero_inactive) {
+      uint4* zr = reinterpret_cast<uint4*>(reinterpret_cast<T16*>(p.dx) + static_cast<size_t>(row) * H);
+      for (int vi = lane; vi < nvec; vi += 32) zr[vi] = make_uint4(0, 0, 0, 0);
+    }
+    return;
+  }
+  DropoutRng rng;
+  rng.k0 = p.seed_lo; rng.k1 = p.seed_hi; rng.s0 = p.stream_lo; rng.s1 = p.stream_hi;
+  if (p.drop_thr16) rng_add_dev_offset(p.rng_dev, rng.s0, rng.s1);
+  rng.thr16 = p.drop_thr16; rng.inv_keep = p.drop_inv_keep;
   float xv[NV][8], dv[NV][8];
   float sum = 0.f;
 #pragma unroll
@@ -322,6 +333,11 @@ ln_bwd_rows_kernel(const LnBwdParams p, float2* __restrict__ stats) {
                                                           static_cast<size_t>(row) * H) + vi), dv[i]);
 #pragma unroll
       for (int e = 0; e < 8; ++e) sum += xv[i][e];
+      if (p.dy_drop) {               // y = dropout(LN(x)) (deterministic mode only): mask dy
+        const uint4 rnd = rng.draw8((static_cast<uint64_t>(row) * H + vi * 8) >> 3);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) dv[i][e] = (rand16_of(rnd, e) < rng.thr16) ? 0.f : dv[i][e] * rng.inv_keep;
+      }
     }
   }
   const float mean = warp_sum(sum) * inv_h;
@@ -353,10 +369,6 @@ ln_bwd_rows_kernel(const LnBwdParams p, float2* __restrict__ stats) {
   s1 = warp_sum(s1) * inv_h;
   s2 = warp_sum(s2) * inv_h;
   if (lane == 0) stats[row] = make_float2(mean, rstd);
-  DropoutRng rng;
-  rng.k0 = p.seed_lo; rng.k1 = p.seed_hi; rng.s0 = p.stream_lo; rng.s1 = p.stream_hi;
-  if (p.drop_thr16) rng_add_dev_offset(p.rng_dev, rng.s0, rng.s1);
-  rng.thr16 = p.drop_thr16; rng.inv_keep = p.drop_inv_keep;
   uint4* dxr = reinterpret_cast<uint4*>(reinterpret_cast<T16*>(p.dx) + static_cast<size_t>(row) * H);
   uint4* ddr = p.dx_drop ? reinterpret_cast<uint4*>(reinterpret_cast<T16*>(p.dx_drop) + static_cast<size_t>(row) * H)
                          : nullptr;
@@ -438,6 +450,60 @@ ln_bwd_cols_kernel(const LnBwdParams p, const float2* __restrict__ stats, int ro
   }
 }
 
+// Deterministic form of ln_bwd_cols_kernel: CTA = 8 columns x 256 row lanes over ALL rows, so every
+// column has one owner and a fixed summation order (det_tree_sum8).  Also covers the row-kind and
+// dropout-on-dy cases of the embedding front-end (the fused kernel's job in the default mode).
+template <bool kBF16>
+__global__ void __launch_bounds__(256, 1)   // (256) alone: ptxas caps it at 64 registers and spills
+ln_bwd_cols_det_kernel(const LnBwdParams p, const float2* __restrict__ stats) {
+  pdl_launch_dependents();
+  pdl_wait();
+  using T16 = typename Elem<kBF16>::T;
+  __shared__ float red[256][9];
+  const int col0 = blockIdx.x * 8;
+  const int H = p.H;
+  const void* lin = p.dx_drop ? p.dx_drop : p.dx;
+  DropoutRng rng;
+  rng.k0 = p.seed_lo; rng.k1 = p.seed_hi; rng.s0 = p.stream_lo; rng.s1 = p.stream_hi;
+  if (p.drop_thr16) rng_add_dev_offset(p.rng_dev, rng.s0, rng.s1);
+  rng.thr16 = p.drop_thr16; rng.inv_keep = p.drop_inv_keep;
+  float ag[8], ab[8], ad[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) { ag[e] = 0.f; ab[e] = 0.f; ad[e] = 0.f; }
+  for (int r = threadIdx.x; r < p.rows; r += 256) {
+    if (p.row_kind != nullptr && p.row_kind[r] != p.kind) continue;
+    const float2 st = __ldg(stats + r);
+    float x[8], dy[8];
+    const size_t off = static_cast<size_t>(r) * H + col0;
+    unpack8<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.x) + off)), x);
+    unpack8<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.dy) + off)), dy);
+    if (p.dy_drop) {
+      const uint4 rnd = rng.draw8(off >> 3);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) dy[e] = (rand16_of(rnd, e) < rng.thr16) ? 0.f : dy[e] * rng.inv_keep;
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      ag[e] = fmaf(dy[e], (x[e] - st.x) * st.y, ag[e]);
+      ab[e] += dy[e];
+    }
+    if (p.dbias) {
+      float d[8];
+      unpack8<kBF16>(*reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(lin) + off), d);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) ad[e] += d[e];
+    }
+  }
+  const float sg = det_tree_sum8(ag, red);
+  const float sb = det_tree_sum8(ab, red);
+  const float sd = det_tree_sum8(ad, red);
+  if (threadIdx.x < 8) {
+    p.dgamma[col0 + threadIdx.x] += sg;
+    p.dbeta[col0 + threadIdx.x] += sb;
+    if (p.dbias) p.dbias[col0 + threadIdx.x] += sd;
+  }
+}
+
 // ------------------------------------------------------------------------------ gather rows
 template <int kDummy>
 __global__ void __launch_bounds__(256)
@@ -497,6 +563,29 @@ colsum_kernel(const void* __restrict__ x_, float* __restrict__ out, int rows, in
       atomicAdd(reinterpret_cast<float4*>(out + col), make_float4(s[0], s[1], s[2], s[3]));
     }
   }
+}
+
+// Deterministic column sum: CTA = 8 columns x 256 row lanes over all rows (see det_tree_sum8).
+template <bool kBF16>
+__global__ void __launch_bounds__(256)
+colsum_det_kernel(const void* __restrict__ x_, float* __restrict__ out, int rows, long long ld,
+                  const int* __restrict__ rows_dev) {
+  pdl_launch_dependents();
+  pdl_wait();
+  if (rows_dev != nullptr) rows = min(rows, *rows_dev);
+  using T16 = typename Elem<kBF16>::T;
+  __shared__ float red[256][9];
+  const int col0 = blockIdx.x * 8;
+  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int r = threadIdx.x; r < rows; r += 256) {
+    float f[8];
+    unpack8<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(x_) +
+                                                        static_cast<size_t>(r) * ld + col0)), f);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[e] += f[e];
+  }
+  const float s = det_tree_sum8(acc, red);
+  if (threadIdx.x < 8) out[col0 + threadIdx.x] += s;
 }
 
 // ------------------------------------------------------------------------------ fp32 -> 16-bit
@@ -583,6 +672,14 @@ int launch_ln_bwd_split(int dtype, const LnBwdParams& p, float* stats_ws, cudaSt
     if (bf) UB_CHECK_CUDA(launch_ln_bwd_rows_nv<true>(p, stats, grid, stream));
     else UB_CHECK_CUDA(launch_ln_bwd_rows_nv<false>(p, stats, grid, stream));
   }
+  if (deterministic()) {
+    ProfScope ps(stream);
+    if (bf) UB_CHECK_CUDA(launch_pdl(ln_bwd_cols_det_kernel<true>, dim3(p.H / 8), dim3(256), 0, stream, 1, p,
+                                     static_cast<const float2*>(stats)));
+    else UB_CHECK_CUDA(launch_pdl(ln_bwd_cols_det_kernel<false>, dim3(p.H / 8), dim3(256), 0, stream, 1, p,
+                                  static_cast<const float2*>(stats)));
+    return 0;
+  }
   {
     const int gx = (p.H + 63) / 64;
     int gy = (2 * num_sms() + gx - 1) / gx;
@@ -625,9 +722,20 @@ int launch_gather_rows(const void* src, void* dst, const int* idx, int rows, int
   return 0;
 }
 
+int launch_colsum_det(int dtype, const void* x, float* out, int rows, int N, long long ld, cudaStream_t stream,
+                      const int* rows_dev) {
+  if (N % 8 != 0 || ld % 8 != 0 || rows <= 0)
+    return set_error(UB200_EINVAL, "colsum: rows > 0, N %% 8 == 0, ld %% 8 == 0 required");
+  ProfScope ps(stream);
+  if (dtype == UB200_BF16) UB_CHECK_CUDA(launch_pdl(colsum_det_kernel<true>, dim3(N / 8), dim3(256), 0, stream, 1, x, out, rows, ld, rows_dev));
+  else UB_CHECK_CUDA(launch_pdl(colsum_det_kernel<false>, dim3(N / 8), dim3(256), 0, stream, 1, x, out, rows, ld, rows_dev));
+  return 0;
+}
+
 int launch_colsum(int dtype, const void* x, float* out, int rows, int N, int ld, cudaStream_t stream) {
   if (N % 8 != 0 || ld % 8 != 0 || rows <= 0)
     return set_error(UB200_EINVAL, "colsum: rows > 0, N %% 8 == 0, ld %% 8 == 0 required");
+  if (deterministic()) return launch_colsum_det(dtype, x, out, rows, N, ld, stream);
   const int gx = (N + 255) / 256;
   int gy = (2 * num_sms() + gx - 1) / gx;
   if (gy > (rows + 31) / 32) gy = (rows + 31) / 32;
@@ -715,6 +823,14 @@ extern "C" int ub200_layernorm_bwd(const ub200_ln_bwd_args* a, ub200_stream_t st
   p.stream_lo = static_cast<uint32_t>(a->rng_stream);
   p.stream_hi = static_cast<uint32_t>(a->rng_stream >> 32);
   p.rng_dev = reinterpret_cast<const unsigned long long*>(a->rng_offset_dev);
+  if (ub::deterministic()) {   // one form for every case: row kernel + fixed-order column kernel
+    UB_CHECK_ARG(a->stats_ws != nullptr, "layernorm_bwd: deterministic mode needs stats_ws (rows x 2 floats)");
+    UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
+    if (p.H % 8 != 0 || p.H > ub::LN_MAX_VEC * 256 || p.rows <= 0)
+      return ub::set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
+                           ub::LN_MAX_VEC * 256, p.H);
+    return ub::launch_ln_bwd_split(a->dtype, p, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
+  }
   if (a->stats_ws != nullptr && a->row_kind == nullptr && !p.dy_drop) {
     UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
     if (p.H % 8 != 0 || p.H > ub::LN_MAX_VEC * 256 || p.rows <= 0)

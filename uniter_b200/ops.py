@@ -156,7 +156,7 @@ def layernorm_bwd(dy, x, gamma, dropout_p=0.0, rng_seed=0, rng_stream=0, want_db
                   row_kind=None, kind=0, dropout_on_dy=False, dx=None, dgamma=None, dbeta=None, dbias=None,
                   zero_inactive=False, rng_offset_dev=None, split=False):
     """Returns dx, dx_drop (or None), dgamma, dbeta, dbias (fp32).  split=True: row kernel + column
-    kernel (plain case only)."""
+    kernel (plain case only; in the deterministic mode every case is split)."""
     lib = _lib.load()
     rows, H = x.shape
     if dx is None:
@@ -175,7 +175,7 @@ def layernorm_bwd(dy, x, gamma, dropout_p=0.0, rng_seed=0, rng_stream=0, want_db
                        row_kind=_lib.ptr(row_kind), kind=int(kind),
                        dropout_on_dy=(1 if dropout_on_dy else 0) | (2 if zero_inactive else 0),
                        rng_offset_dev=rng_offset_dev)
-    if split:
+    if split or _lib.deterministic():   # the deterministic mode always takes the split form
         ws = torch.empty(rows, 2, device=x.device, dtype=torch.float32)
         a.stats_ws = ws.data_ptr()
     _lib.check(lib.ub200_layernorm_bwd(C.byref(a), _lib.current_stream()))

@@ -298,8 +298,11 @@ class FusedAdamW(object):
         self._lr_events = [None] * 4
         self._lr_last = None
         self.last_sumsq = torch.zeros(1, device=dev, dtype=torch.float32)
+        # one fp32 partial per block: the fixed-order sum of squares of the deterministic mode
+        sumsq_ws = torch.empty(max(_lib.load().ub200_grad_sumsq_workspace_bytes(nblocks) // 4, 1), device=dev,
+                               dtype=torch.float32)
         self._tables = dict(key=key, segs=segs_dev, starts=starts_dev, nseg=nseg, nblocks=nblocks,
-                            betas=betas, eps=eps, keep=keep)
+                            betas=betas, eps=eps, keep=keep, sumsq_ws=sumsq_ws)
         return self._tables
 
     def prepare(self):
@@ -356,8 +359,7 @@ class FusedAdamW(object):
             self.sync_lr()
         stream = _lib.current_stream()
         self.last_sumsq.zero_()
-        _lib.check(lib.ub200_grad_sumsq(T["segs"].data_ptr(), T["starts"].data_ptr(), T["nseg"], T["nblocks"],
-                                        self.last_sumsq.data_ptr(), stream))
+        self._grad_sumsq(lib, T, stream)
         _lib.check(lib.ub200_adam_prep(self.last_sumsq.data_ptr(), self._dev_state.data_ptr(), stream))
         clip = max_grad_norm is not None and max_grad_norm > 0
         _lib.check(lib.ub200_adamw_step(T["segs"].data_ptr(), T["starts"].data_ptr(), T["nseg"], T["nblocks"],
@@ -365,6 +367,11 @@ class FusedAdamW(object):
                                         float(max_grad_norm) if clip else -1.0, self.last_sumsq.data_ptr(),
                                         self._dev_state.data_ptr(), self._lr_dev.data_ptr(), stream))
         return None
+
+    def _grad_sumsq(self, lib, T, stream):
+        ws = T["sumsq_ws"]
+        _lib.check(lib.ub200_grad_sumsq_ws(T["segs"].data_ptr(), T["starts"].data_ptr(), T["nseg"], T["nblocks"],
+                                           self.last_sumsq.data_ptr(), ws.data_ptr(), ws.numel() * 4, stream))
 
     def _step_scaled(self, lib, scaler, loss_id, max_grad_norm):
         scaler._check_id(loss_id)
@@ -381,8 +388,7 @@ class FusedAdamW(object):
             self.sync_lr()
         stream = _lib.current_stream()
         self.last_sumsq.zero_()
-        _lib.check(lib.ub200_grad_sumsq(T["segs"].data_ptr(), T["starts"].data_ptr(), T["nseg"], T["nblocks"],
-                                        self.last_sumsq.data_ptr(), stream))
+        self._grad_sumsq(lib, T, stream)
         _lib.check(lib.ub200_adam_prep_scaled(self.last_sumsq.data_ptr(), self._dev_state.data_ptr(),
                                               scaler.table.data_ptr(), loss_id, stream))
         clip = max_grad_norm is not None and max_grad_norm > 0
