@@ -57,8 +57,9 @@ int ub200_set_sm_reserve(int n);
 /* Deterministic mode (on != 0; returns the previous value).  Read at launch time, like the SM reserve,
  * so a captured CUDA graph keeps the mode it was captured under.  With the mode on, the reductions
  * below use no floating-point atomics and no summation order that depends on the grid (so neither the
- * SM reserve nor appended all-zero padding rows change their bits).  A whole training step is not yet
- * bit-reproducible in this mode (see DESIGN.md section 3b).  The forms it selects:
+ * SM reserve nor appended all-zero padding rows change their bits): a whole training step with
+ * sequences of at most 128 tokens is bit-reproducible in this mode.  The Python package sets it from
+ * torch.use_deterministic_algorithms (see DESIGN.md section 3b).  The forms it selects:
  *   column sums (ub200_colsum, UB200_EPI_COLSUM, the attention's dbias, the LayerNorm backward's
  *     dgamma / dbeta / dbias, ub200_embed_bwd_colsums): one CTA owns 8 columns, thread t sums rows
  *     t, t + 256, ... in ascending order, the 256 partials meet in a fixed tree;
@@ -454,7 +455,7 @@ typedef struct {
   int32_t skipped;    /* number of skipped (overflowed) steps */
   int32_t _pad;
 } ub200_adam_state;
-int ub200_adam_prep(const float* sumsq, ub200_adam_state* state_dev, ub200_stream_t stream);
+int ub200_adam_prep(const float* sumsq, ub200_adam_state* state_dev, ub200_stream_t stream);  /* ordinary launch, no PDL */
 enum { UB200_F32 = 2 };
 int32_t ub200_adam_chunk(void);
 int ub200_grad_sumsq(const ub200_adam_segment* segs_dev, const int32_t* blk_start_dev, int32_t nseg,

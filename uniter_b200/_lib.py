@@ -3,7 +3,9 @@
 There is deliberately no fallback: if the library is missing or the device is not sm_90 the
 import of the compute path raises.
 """
+import contextlib
 import ctypes as C
+import functools
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -241,6 +243,81 @@ def ptr(t):
 def deterministic():
     """Whether the library's deterministic mode (ub200_set_deterministic) is on: read from the library."""
     return bool(load().ub200_deterministic())
+
+
+# Longest sequence whose attention backward has a fixed-order form (attn.cu: SH_MAXSEQ).  Longer
+# sequences sum dQ over key blocks with float atomics; the deterministic mode refuses them.
+DET_ATTN_BWD_MAX_SEQLEN = 128
+
+_pinned_modes = []      # modes of the enclosing library_mode() scopes, innermost last
+
+
+def select_mode(max_seqlen=None):
+    """The library mode for launches made here: the one place where torch's determinism flags are read.
+
+    Returns None when torch.use_deterministic_algorithms is off (the library's switch is left as it is,
+    so C callers and tests that set it keep their mode), 1 when it is on, and 0 for work the fixed-order
+    mode cannot cover under warn_only.  Inside a library_mode() scope (an autograd backward, a captured
+    step) the scope's mode is returned instead of reading torch's flags again.
+
+    max_seqlen: the host-known longest sequence of work that includes an attention backward.  Above
+    DET_ATTN_BWD_MAX_SEQLEN the mode has no fixed-order form: this raises a RuntimeError, or with
+    warn_only=True warns and returns 0 (that work runs in the default mode)."""
+    import torch
+    if _pinned_modes:
+        mode = _pinned_modes[-1]
+    else:
+        mode = 1 if torch.are_deterministic_algorithms_enabled() else None
+    if mode == 1 and max_seqlen is not None and max_seqlen > DET_ATTN_BWD_MAX_SEQLEN:
+        msg = ("libub200 attention backward with max_seqlen %d > %d has no deterministic implementation "
+               "(dQ is summed over key blocks with float atomics); it is refused under "
+               "torch.use_deterministic_algorithms(True)" % (max_seqlen, DET_ATTN_BWD_MAX_SEQLEN))
+        if not torch.is_deterministic_algorithms_warn_only_enabled():
+            raise RuntimeError(msg + ".  Pass warn_only=True to run it in the default mode with a warning.")
+        import warnings
+        warnings.warn(msg + "; with warn_only=True it runs in the default mode.", UserWarning, stacklevel=3)
+        return 0
+    return mode
+
+
+@contextlib.contextmanager
+def library_mode(mode):
+    """Run the enclosed launches in `mode` (a select_mode() result) and restore the previous value of
+    the library's switch afterwards.  None leaves the switch untouched."""
+    lib = load() if mode is not None else None
+    prev = lib.ub200_set_deterministic(mode) if mode is not None else None
+    _pinned_modes.append(mode)
+    try:
+        yield
+    finally:
+        _pinned_modes.pop()
+        if mode is not None:
+            lib.ub200_set_deterministic(prev)
+
+
+def forward_in_mode(max_seqlen=None):
+    """Decorator for the forward of a torch.autograd.Function that launches library work: runs it in
+    select_mode() and stores that mode in ctx for backward_in_mode.  max_seqlen(ctx, *args): the
+    longest sequence whose attention backward this node will run, or None."""
+    def wrap(fn):
+        @functools.wraps(fn)
+        def forward(ctx, *args):
+            mode = select_mode(max_seqlen(ctx, *args) if max_seqlen is not None else None)
+            ctx.ub200_mode = mode
+            with library_mode(mode):
+                return fn(ctx, *args)
+        return forward
+    return wrap
+
+
+def backward_in_mode(fn):
+    """Decorator for the backward of a Function whose forward has forward_in_mode: the backward runs in
+    the mode of its forward, whatever torch's flags are when it runs."""
+    @functools.wraps(fn)
+    def backward(ctx, *grads):
+        with library_mode(ctx.ub200_mode):
+            return fn(ctx, *grads)
+    return backward
 
 
 def current_stream():

@@ -240,10 +240,9 @@ struct AdamHyper {
 
 __device__ __forceinline__ bool sumsq_finite(float s) { return (s == s) && (fabsf(s) <= 3.0e38f); }
 
-// found_inf / step bookkeeping on the device (one thread), between sumsq_kernel and adamw_kernel
+// found_inf / step bookkeeping on the device (one thread), between sumsq_kernel and adamw_kernel.
+// No griddepcontrol, like adam_prep_scaled_kernel: an ordinary launch that never triggers early.
 __global__ void adam_prep_kernel(const float* __restrict__ sumsq, ub200_adam_state* __restrict__ st) {
-  pdl_launch_dependents();
-  pdl_wait();
   const bool finite = sumsq_finite(*sumsq);
   st->found_inf = finite ? 0 : 1;
   if (finite) st->step += 1; else st->skipped += 1;
@@ -495,7 +494,10 @@ extern "C" int ub200_adam_prep(const float* sumsq, ub200_adam_state* state_dev, 
   UB_CHECK_ARG(sumsq && state_dev, "adam_prep: null pointer");
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ProfScope ps(stream);
-  UB_CHECK_CUDA(launch_pdl(adam_prep_kernel, dim3(1), dim3(1), 0, stream, 1, sumsq, state_dev));
+  // An ordinary launch, for the reason given in ub200_adam_prep_scaled: chained by PDL inside a
+  // captured graph, found_inf and the clip factor could read an incomplete sum of squares.
+  adam_prep_kernel<<<1, 1, 0, stream>>>(sumsq, state_dev);
+  UB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 

@@ -123,7 +123,8 @@ class PeerExchange(object):
         a = self._args.get(key)
         if a is None:
             a = self._args[key] = self._make(lo, hi, max_ctas)
-        _lib.check(self.lib.ub200_peer_allreduce(a, _lib.current_stream()))
+        with _lib.library_mode(_lib.select_mode()):
+            _lib.check(self.lib.ub200_peer_allreduce(a, _lib.current_stream()))
         self.calls += 1
 
     def error_word(self):

@@ -17,7 +17,11 @@ What makes the step capturable here:
   * the token count is padded to a bucket (`token_bucket`, default 128 rows = one GEMM row tile) with
     ONE dummy sequence (see model._prefix_pack_host): identical results, bit for bit, and one graph
     serves every batch of the bucket.  The key of a graph is
-    (tensor shapes of the batch, padded token count, attention max-seqlen bucket, accumulate flag).
+    (tensor shapes of the batch, padded token count, attention max-seqlen bucket, accumulate flag,
+    library mode).
+  * the library's deterministic mode follows torch.use_deterministic_algorithms at stage() time
+    (uniter_b200._lib.select_mode): warm-up and capture run in it, and a graph only replays in the
+    mode it was captured in.
 
 Usage:
     step = GraphedStep(model, lambda b: model(b).sum() * b["mlm_inv_n"])
@@ -28,6 +32,7 @@ Usage:
 import numpy as np
 import torch
 
+from . import _lib
 from . import model as _model
 from .arena import GradArena
 
@@ -38,7 +43,7 @@ def _round_up(v, m):
 
 class _Bucket(object):
     __slots__ = ("graph", "graphs", "ship_after", "inputs", "meta_dev", "meta_offs", "loss", "T_pad", "maxseq",
-                 "n_replays", "launches")
+                 "n_replays", "launches", "mode")
 
 
 class GraphedStep(object):
@@ -96,7 +101,15 @@ class GraphedStep(object):
         maxseq = _round_up(max(max(lens), 1, T_pad - T), 128)
         sig = tuple((k, tuple(v.shape), str(v.dtype)) for k, v in sorted(host_batch.items())
                     if torch.is_tensor(v))
-        return (sig, T_pad, maxseq, bool(accumulate), tag, self._steps_optimizer(step_optimizer)), T_pad, maxseq
+        # the library mode the step runs in (torch.use_deterministic_algorithms) and, for a bucket whose
+        # attention backward has no fixed-order form, the warn_only decision (raises, or warns and gives 0:
+        # the encoder node then runs in the default mode, as in an eager step, the rest of the step in the
+        # step's mode).  Both are part of the key, so a change of torch's flags captures a new graph
+        # instead of replaying one of the other mode.
+        long_decision = _lib.select_mode(maxseq)
+        mode = _lib.select_mode()
+        return (sig, T_pad, maxseq, bool(accumulate), tag, self._steps_optimizer(step_optimizer), mode,
+                long_decision), T_pad, maxseq
 
     def _steps_optimizer(self, step_optimizer):
         return self.optimizer is not None and bool(step_optimizer)
@@ -124,6 +137,10 @@ class GraphedStep(object):
 
     # ------------------------------------------------------------------ the captured region
     def _run(self, bk, accumulate, tag=None, step_optimizer=True):
+        with _lib.library_mode(bk.mode):
+            return self._run_in_mode(bk, accumulate, tag, step_optimizer)
+
+    def _run_in_mode(self, bk, accumulate, tag, step_optimizer):
         self.rng_counter.add_(64)                       # fresh dropout masks for this replay
         self.arena.begin_step(accumulate=accumulate, zero_all=self.zero_all)
         _model._RNG_GRAPH["dev"] = self.rng_counter
@@ -152,7 +169,7 @@ class GraphedStep(object):
 
     def _capture(self, key, host_batch, lens, T_pad, maxseq, accumulate, tag=None, step_optimizer=True):
         bk = _Bucket()
-        bk.T_pad, bk.maxseq, bk.n_replays = T_pad, maxseq, 0
+        bk.T_pad, bk.maxseq, bk.n_replays, bk.mode = T_pad, maxseq, 0, key[-2]
         dev = self.device
         bk.inputs = {k: torch.empty(v.shape, dtype=v.dtype, device=dev)
                      for k, v in host_batch.items() if torch.is_tensor(v)}
@@ -194,7 +211,6 @@ class GraphedStep(object):
             opt.prepare()
         if self.pool is None:
             self.pool = torch.cuda.graph_pool_handle()
-        from . import _lib
         lib = _lib.load()
         lib.ub200_launch_count.restype = __import__("ctypes").c_ulonglong
         n0 = lib.ub200_launch_count()

@@ -20,7 +20,7 @@ import torch
 from torch import nn
 from torch.nn import functional as F
 
-from . import ops
+from . import _lib, ops
 from .model import LibLinear, UniterModel, UniterPreTrainedModel, gather_packed_rows
 
 
@@ -74,6 +74,7 @@ class _MlmHead(torch.autograd.Function):
     buffer that the decoder wgrad writes first and the embedding scatter adds to later)."""
 
     @staticmethod
+    @_lib.forward_in_mode()
     def forward(ctx, h, module, targets, want_scores):
         p = module.cls.predictions
         dense_w, dense_b = p.transform.dense.weight, p.transform.dense.bias
@@ -104,6 +105,7 @@ class _MlmHead(torch.autograd.Function):
         return loss
 
     @staticmethod
+    @_lib.backward_in_mode
     def backward(ctx, dloss):
         from .arena import GradArena
         h, pre, t, z, logits, lse, targets = ctx.saved_tensors
@@ -181,6 +183,7 @@ class LibTransform(torch.autograd.Function):
     written there directly."""
 
     @staticmethod
+    @_lib.forward_in_mode()
     def forward(ctx, h, dense_w, dense_b, ln_g, ln_b):
         h = h.contiguous()
         t, pre = ops.gemm(h, dense_w, bias=dense_b, gelu=True)
@@ -190,6 +193,7 @@ class LibTransform(torch.autograd.Function):
         return z
 
     @staticmethod
+    @_lib.backward_in_mode
     def backward(ctx, dz):
         h, pre, t = ctx.saved_tensors
         dense_w, dense_b, ln_g, ln_b = ctx.params

@@ -432,6 +432,7 @@ class _GatherRows(torch.autograd.Function):
     back, so duplicates in an arbitrary gather_index accumulate like torch.gather's backward."""
 
     @staticmethod
+    @_lib.forward_in_mode()
     def forward(ctx, src, index, n_src_rows, inverse):
         lib = _bind()
         src = src.contiguous()
@@ -447,6 +448,7 @@ class _GatherRows(torch.autograd.Function):
         return dst
 
     @staticmethod
+    @_lib.backward_in_mode
     def backward(ctx, grad):
         (index,) = ctx.saved_tensors
         grad = grad.contiguous()
@@ -474,6 +476,7 @@ class LibLinear(torch.autograd.Function):
     written there directly (None is returned to autograd); others are returned normally."""
 
     @staticmethod
+    @_lib.forward_in_mode()
     def forward(ctx, x, weight, bias, w_kn, tanh):
         from . import ops
         if not x.is_cuda or x.dtype not in (torch.float16, torch.bfloat16):
@@ -498,6 +501,7 @@ class LibLinear(torch.autograd.Function):
         return out[:, :N] if Np != N else out
 
     @staticmethod
+    @_lib.backward_in_mode
     def backward(ctx, dy):
         from . import ops
         x2, w, y = ctx.saved_tensors
@@ -549,6 +553,7 @@ class _EmbedFront(torch.autograd.Function):
     requires-grad handle that makes autograd call backward."""
 
     @staticmethod
+    @_lib.forward_in_mode()
     def forward(ctx, anchor, model, meta, mode, input_ids, position_ids, img_feat, img_pos_feat,
                 gather_index, img_masks, txt_type_ids, img_type_ids, dropout_p):
         from . import ops
@@ -619,6 +624,7 @@ class _EmbedFront(torch.autograd.Function):
         return x
 
     @staticmethod
+    @_lib.backward_in_mode
     def backward(ctx, dx):
         """Row-kind masked LayerNorm backward (x4), img_linear wgrad on the wgmma GEMM, then the
         table gradients in three launches (ub200_embed_bwd_scatter / _colsums); every small fp32
@@ -710,6 +716,8 @@ class _EncoderStack(torch.autograd.Function):
     """NL x BertLayer over packed tokens: one C-ABI call forward, one backward."""
 
     @staticmethod
+    @_lib.forward_in_mode(
+        lambda ctx, x, anchor, model, meta, want_all, need_grad: meta["max_seqlen"] if need_grad else None)
     def forward(ctx, x, anchor, model, meta, want_all, need_grad):
         lib = _bind()
         cfg = model.config
@@ -747,6 +755,7 @@ class _EncoderStack(torch.autograd.Function):
         return outs[NL - 1]
 
     @staticmethod
+    @_lib.backward_in_mode
     def backward(ctx, grad_out):
         lib = _bind()
         model = ctx.model

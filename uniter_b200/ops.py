@@ -4,6 +4,7 @@ These allocate outputs with torch (the ABI never allocates), pass raw pointers a
 torch's current CUDA stream.  No torch math happens here.
 """
 import ctypes as C
+import functools
 
 import torch
 
@@ -12,6 +13,17 @@ from ._lib import (EPI_ACCUM, EPI_ATOMIC, EPI_BIAS, EPI_COLSUM, EPI_DGELU, EPI_D
                    EPI_OUT_F32, EPI_RESIDUAL)
 
 
+def _follows_torch(fn):
+    """Launch in the mode _lib.select_mode() gives at the call: torch.use_deterministic_algorithms, or
+    inside an autograd backward the mode of its forward."""
+    @functools.wraps(fn)
+    def call(*args, **kwargs):
+        with _lib.library_mode(_lib.select_mode()):
+            return fn(*args, **kwargs)
+    return call
+
+
+@_follows_torch
 def gemm(a, b, *, a_major=0, b_major=0, bias=None, residual=None, aux=None, out=None,
          gelu=False, dgelu=False, accumulate=False, out_fp32=False, colsum=None,
          dropout_p=0.0, rng_seed=0, rng_stream=0, tile_n=0, max_ctas=0, cluster=0, k_splits=0,
@@ -103,6 +115,7 @@ def _out_buffer(buf, shape, like, dtype):
     return buf
 
 
+@_follows_torch
 def attn_fwd(qkv, cu_seqlens, max_seqlen, num_heads, dropout_p=0.0, rng_seed=0, rng_stream=0,
              rng_offset_dev=None, ctx=None, lse=None):
     """ctx [T, H], lse [heads, T] = fused varlen attention over packed qkv [T, 3H].
@@ -124,7 +137,15 @@ def attn_fwd(qkv, cu_seqlens, max_seqlen, num_heads, dropout_p=0.0, rng_seed=0, 
 def attn_bwd(qkv, ctx, lse, dctx, cu_seqlens, max_seqlen, num_heads, dropout_p=0.0, rng_seed=0,
              rng_stream=0, dbias=None, rng_offset_dev=None, dqkv=None):
     """dqkv [T, 3H] of attn_fwd; dbias [3H] fp32, if given, is accumulated into (column sums of dqkv).
-    dqkv: optional preallocated output (written, not accumulated into)."""
+    dqkv: optional preallocated output (written, not accumulated into).  Under
+    torch.use_deterministic_algorithms, max_seqlen > 128 raises (warn_only: runs in the default mode)."""
+    with _lib.library_mode(_lib.select_mode(max_seqlen)):
+        return _attn_bwd(qkv, ctx, lse, dctx, cu_seqlens, max_seqlen, num_heads, dropout_p, rng_seed,
+                         rng_stream, dbias, rng_offset_dev, dqkv)
+
+
+def _attn_bwd(qkv, ctx, lse, dctx, cu_seqlens, max_seqlen, num_heads, dropout_p, rng_seed, rng_stream,
+              dbias, rng_offset_dev, dqkv):
     lib = _lib.load()
     T, H3 = qkv.shape
     H = H3 // 3
@@ -143,6 +164,7 @@ def attn_bwd(qkv, ctx, lse, dctx, cu_seqlens, max_seqlen, num_heads, dropout_p=0
     return dqkv
 
 
+@_follows_torch
 def layernorm_fwd(x, gamma, beta):
     lib = _lib.load()
     rows, H = x.shape
@@ -152,6 +174,7 @@ def layernorm_fwd(x, gamma, beta):
     return y
 
 
+@_follows_torch
 def layernorm_bwd(dy, x, gamma, dropout_p=0.0, rng_seed=0, rng_stream=0, want_dbias=True,
                   row_kind=None, kind=0, dropout_on_dy=False, dx=None, dgamma=None, dbeta=None, dbias=None,
                   zero_inactive=False, rng_offset_dev=None, split=False):
@@ -182,6 +205,7 @@ def layernorm_bwd(dy, x, gamma, dropout_p=0.0, rng_seed=0, rng_stream=0, want_db
     return dx, dx_drop, dgamma, dbeta, dbias
 
 
+@_follows_torch
 def colsum(x, out=None):
     lib = _lib.load()
     rows, N = x.shape
@@ -192,6 +216,7 @@ def colsum(x, out=None):
     return out
 
 
+@_follows_torch
 def cvt_from_f32(src, dtype, out=None, accumulate=False):
     """16-bit copy of an fp32 tensor (one launch)."""
     lib = _lib.load()
@@ -205,6 +230,7 @@ def cvt_from_f32(src, dtype, out=None, accumulate=False):
     return out
 
 
+@_follows_torch
 def ce_fwd(logits, targets, vocab):
     """loss [n] fp32, lse [n] fp32 of softmax cross-entropy over logits[:, :vocab] (16-bit, row
     pitch a multiple of 8)."""
@@ -219,6 +245,7 @@ def ce_fwd(logits, targets, vocab):
     return loss, lse
 
 
+@_follows_torch
 def ce_bwd_(logits, targets, lse, dloss, vocab):
     """In place: logits[:, c] <- (softmax - onehot) * dloss for c < vocab, 0 for the padding columns."""
     lib = _lib.load()
@@ -230,6 +257,7 @@ def ce_bwd_(logits, targets, lse, dloss, vocab):
     return logits
 
 
+@_follows_torch
 def dgelu_mul(dy, pre):
     lib = _lib.load()
     out = torch.empty_like(dy)
@@ -239,6 +267,7 @@ def dgelu_mul(dy, pre):
     return out
 
 
+@_follows_torch
 def dtanh_mul(dy, y):
     """dy * (1 - y^2): backward of y = tanh(.) (BertPooler)."""
     lib = _lib.load()
@@ -249,6 +278,7 @@ def dtanh_mul(dy, y):
     return out
 
 
+@_follows_torch
 def gather_rows(src, index, rows=None):
     """dst[r] = src[index[r]] if index[r] >= 0 else 0 (int32 index; bit-exact row mover)."""
     lib = _lib.load()

@@ -114,6 +114,41 @@ class DynamicLossScaler(object):
         self.table.copy_(scaler_table(entries))        # in place: the table keeps its address
 
 
+def _owned_ranges(params):
+    """For each parameter, the element ranges [lo, hi) of its storage that its own segment updates.
+
+    Parameters may share storage: UniterForImageTextRetrieval.init_output() makes rank_output.weight and
+    .bias views of row 1 of itm_output's.  Every element of model storage is updated by ONE segment per
+    step, that of the innermost parameter covering it (of parameters with the same range, the first
+    listed), so no two CTAs of one launch write the same address, and a view's elements follow the view's
+    own gradient and moments.  The covering parameter's gradient over those elements is not used, and
+    they are left out of its share of the gradient norm.  Storage that two parameters share only in part
+    has no single owner and is refused."""
+    spans = [(p.data_ptr(), p.data_ptr() + p.numel() * p.element_size(), p.element_size()) for p in params]
+    out = []
+    for i, (lo, hi, es) in enumerate(spans):
+        holes = []
+        for j, (lo2, hi2, es2) in enumerate(spans):
+            if j == i or hi2 <= lo or hi <= lo2:
+                continue
+            inside, around = lo <= lo2 and hi2 <= hi, lo2 <= lo and hi <= hi2
+            if not (inside or around) or es2 != es or (lo2 - lo) % es:
+                raise RuntimeError("FusedAdamW: parameters %d and %d share storage in part; give each shared "
+                                   "element one parameter" % (i, j))
+            if inside and ((lo2, hi2) != (lo, hi) or j < i):
+                holes.append(((lo2 - lo) // es, (hi2 - lo) // es))
+        ranges, cur = [], 0
+        for a, b in sorted(holes):
+            if a > cur:
+                ranges.append((cur, a))
+            cur = max(cur, b)
+        n = (hi - lo) // es
+        if cur < n:
+            ranges.append((cur, n))
+        out.append(ranges)
+    return out
+
+
 class FusedAdamW(object):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-6, weight_decay=0.0,
                  correct_bias=True):
@@ -240,7 +275,8 @@ class FusedAdamW(object):
         return tuple(key)
 
     def _build_tables(self, key):
-        """Segment table (one entry per parameter tensor with a gradient), CTA prefix sums, per-group
+        """Segment table (one entry per range of a parameter with a gradient that the parameter owns, see
+        _owned_ranges: one per parameter unless parameters share storage), CTA prefix sums, per-group
         learning rates and the optimizer state counters, all in DEVICE memory at fixed addresses, so
         that a step is three launches with constant arguments (capturable in a CUDA graph).  Rebuilt
         only when the set of (parameter, gradient buffer) pairs changes."""
@@ -261,6 +297,7 @@ class FusedAdamW(object):
         if self._dev_state is None or self._dev_state.device != dev:
             self._dev_state = torch.zeros(4, device=dev, dtype=torch.int32)
         step_now = self._applied_steps()
+        with_grad = []
         for gi, g in enumerate(self.param_groups):
             b1, b2 = g["betas"]
             if betas is None:
@@ -276,17 +313,25 @@ class FusedAdamW(object):
                     raise RuntimeError("Adam does not support sparse gradients")
                 if not p.is_contiguous() or not p.grad.is_contiguous():
                     raise RuntimeError("FusedAdamW needs contiguous parameters and gradients")
-                st = self._init_state(p, step_now)
+                with_grad.append((gi, g, p))
+        owned = _owned_ranges([p for _, _, p in with_grad])
+        for (gi, g, p), ranges in zip(with_grad, owned):
+            st = self._init_state(p, step_now)
+            ge, me = p.grad.element_size(), p.element_size()
+            for lo, hi in ranges:
                 segs.append(_lib.AdamSegment(
-                    grad=p.grad.data_ptr(), master=st["master"].data_ptr(), exp_avg=st["exp_avg"].data_ptr(),
-                    exp_avg_sq=st["exp_avg_sq"].data_ptr(), model=p.data_ptr(), n=p.numel(),
+                    grad=p.grad.data_ptr() + lo * ge, master=st["master"].data_ptr() + lo * 4,
+                    exp_avg=st["exp_avg"].data_ptr() + lo * 4, exp_avg_sq=st["exp_avg_sq"].data_ptr() + lo * 4,
+                    model=p.data_ptr() + lo * me, n=hi - lo,
                     step_size=0.0, lr_wd=0.0,
                     grad_dtype=_lib.dtype_code(p.grad.dtype, allow_f32=True),
                     model_dtype=_lib.dtype_code(p.dtype, allow_f32=True),
                     weight_decay=float(g["weight_decay"]), group=gi, step_offset=int(st["step_offset"]),
                     flags=1 if g["correct_bias"] else 0))
-                keep.append(p.grad)
-                starts.append(starts[-1] + (p.numel() + chunk - 1) // chunk)
+                starts.append(starts[-1] + (hi - lo + chunk - 1) // chunk)
+            keep.append(p.grad)
+        if not segs:
+            return None
         nseg, nblocks = len(segs), starts[-1]
         arr = (_lib.AdamSegment * nseg)(*segs)
         host = torch.frombuffer(bytearray(C.string_at(C.addressof(arr), C.sizeof(arr))), dtype=torch.uint8)
@@ -345,7 +390,12 @@ class FusedAdamW(object):
         max_grad_norm > 0: clip the global norm of the unscaled gradients like ``clip_grad_norm_``
         (the norm itself stays on the device: ``self.last_sumsq``).  A non-finite norm (fp16
         overflow) SKIPS the step on the device — masters, moments, weights and the step count stay
-        untouched and ``self.found_inf`` is set — like apex's dynamic loss scaler does."""
+        untouched and ``self.found_inf`` is set — like apex's dynamic loss scaler does.
+        Under torch.use_deterministic_algorithms the gradient norm is summed in a fixed order."""
+        with _lib.library_mode(_lib.select_mode()):
+            return self._step(grad_scale, max_grad_norm, loss_id)
+
+    def _step(self, grad_scale, max_grad_norm, loss_id):
         lib = _lib.load()
         if isinstance(grad_scale, DynamicLossScaler):
             return self._step_scaled(lib, grad_scale, int(loss_id), max_grad_norm)
