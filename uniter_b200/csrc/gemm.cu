@@ -16,11 +16,16 @@ int gemm_group_dispatch_f16(const void* tm, const GroupedParams& g, int grid, cu
 int launch_gemm_ln(int dtype, const GemmParams& p, const void* gamma, const void* beta, void* y,
                    long long ldy, const CUtensorMap& tmA, const CUtensorMap& tmB, cudaStream_t stream);
 
-// Pick (N tile, CTAs per tile) minimising  waves x k-blocks x cycles-per-k-block + exposed tail.
-// The cost model is a heuristic: a fixed per-k-block cost plus a part proportional to the tile
-// width (cheaper per column for a 2-CTA cluster, whose B tile is fetched once per pair), so fewer,
-// wider tiles win until wave quantisation bites.  The epilogue of the last tile and a fixed
-// launch / prologue cost are exposed once.  Its constants have not been re-fitted on H100.
+// Pick (N tile, CTAs per tile) minimising the modelled time in microseconds:
+//   waves x (k-blocks x per_kb(bn, cluster) + per_tile(bn, cluster)).
+// per_kb is the mainloop time of one 128 x bn x 64 step; per_tile is the epilogue and the tile
+// switch, which a wave pays once per tile (the producer only prefetches across it).  Both grow with
+// the tile width; a 2-CTA cluster fetches each B tile once per pair.  Wide tiles amortise the fixed
+// part until wave quantisation bites, which is what makes 128-wide tiles win for the N = 3072, K = 768
+// GEMMs at 27 row tiles (648 tiles = 4.9 waves) and 192 / 256 win at 28.  The constants are a
+// non-negative least-squares fit to tools/gemm_roles.py over the eight encoder roles, T = 3456 and 3578,
+// every (tile, cluster) below, on an H100 80GB HBM3 at 700 W (profiles/h100_c2_gemm_tiles.jsonl); the
+// fitted choice is the measured fastest at 15 of those 16 shapes and within 0.2 us at the other.
 static void pick_config(int M, int N, int K, int sms, int* bn_out, int* cluster_out) {
   const int tiles_m = (M + BM - 1) / BM;
   const int num_kb = (K + BK - 1) / BK;
@@ -33,8 +38,9 @@ static void pick_config(int M, int N, int K, int sms, int* bn_out, int* cluster_
     const int units = ((tiles_m + c - 1) / c) * ((N + bn - 1) / bn);
     const int slots = sms / c;
     const int waves = (units + slots - 1) / slots;
-    const double per_kb = (c == 1) ? 421.0 + 1.27 * bn : 552.0 + 0.59 * bn;
-    const double cost = static_cast<double>(waves) * num_kb * per_kb + 25.0 * bn + 3000.0;
+    const double per_kb = (c == 1) ? 0.1298 + 0.00184 * bn : 0.0602 + 0.00217 * bn;
+    const double per_tile = (c == 1) ? 0.3956 + 0.03142 * bn : 0.03538 * bn;
+    const double cost = static_cast<double>(waves) * (num_kb * per_kb + per_tile);
     if (cost < best - 1e-9) { best = cost; *bn_out = bn; *cluster_out = c; }
   }
 }
@@ -226,7 +232,7 @@ extern "C" int ub200_gemm_grouped(const ub200_gemm_args* args, int32_t count, ub
                  "gemm_grouped[%d]: bad shape", i);
   }
   // N tile shared by the group: fewest (rounds over the SMs) x (cost per k-block of a 128 x bn tile,
-  // the same unmeasured heuristic as pick_config's: wider tiles cost less per column).
+  // an unmeasured heuristic, not part of pick_config's fit: wider tiles cost less per column).
   const int sms = num_sms();
   int bn = args[0].tile_n;
   if (bn == 0) {
