@@ -18,14 +18,20 @@ int launch_gemm_ln(int dtype, const GemmParams& p, const void* gamma, const void
 
 // Pick (N tile, CTAs per tile) minimising the modelled time in microseconds:
 //   waves x (k-blocks x per_kb(bn, cluster) + per_tile(bn, cluster)).
-// per_kb is the mainloop time of one 128 x bn x 64 step; per_tile is the epilogue and the tile
-// switch, which a wave pays once per tile (the producer only prefetches across it).  Both grow with
-// the tile width; a 2-CTA cluster fetches each B tile once per pair.  Wide tiles amortise the fixed
-// part until wave quantisation bites, which is what makes 128-wide tiles win for the N = 3072, K = 768
-// GEMMs at 27 row tiles (648 tiles = 4.9 waves) and 192 / 256 win at 28.  The constants are a
-// non-negative least-squares fit to tools/gemm_roles.py over the eight encoder roles, T = 3456 and 3578,
-// every (tile, cluster) below, on an H100 80GB HBM3 at 700 W (profiles/h100_c2_gemm_tiles.jsonl); the
-// fitted choice is the measured fastest at 15 of those 16 shapes and within 0.2 us at the other.
+// per_kb is the mainloop time of one 128 x bn x 64 step; per_tile is what a wave loses per tile
+// beyond its mainloop: the part of the epilogue warpgroup's work that the next mainloop does not
+// hide, and the tile switch.  Both grow with the tile width; a 2-CTA cluster fetches each B tile once
+// per pair.  Wide tiles amortise the fixed part until wave quantisation bites, which is what makes
+// 128-wide tiles win for the N = 3072, K = 768 GEMMs at 27 row tiles (648 tiles = 4.9 waves).
+// The constants are a non-negative least-squares fit (relative error) to tools/gemm_roles.py over the
+// eight encoder roles, T = 3456 and 3578, every (tile, cluster) below, on an H100 80GB HBM3 at 700 W
+// (profiles/h100_c2_gemm_tiles_epilogue_wg.jsonl).  Scored on those explicit-tile timings, the fitted
+// choices total 426.1 us over the 16 shapes against 421.2 us for the fastest tile of each shape.  All
+// of the gap is at 28 row tiles, in the two N = 3072 roles with the erf epilogues (GELU, dGELU),
+// whose tiles are bound by the epilogue warpgroup: there waves x width is the same for 128, 192 and
+// 256 (6, 4 and 3 waves), and the model, which knows only (M, N, K), picks 256 (FFN1 fwd 45.5 us
+// where 128 gives 42.5; FFN2 dgrad 49.9 us where 192 gives 48.0).  The overlapped form,
+// waves x max(mainloop, epilogue) + one epilogue, fitted to the same timings, makes the same choices.
 static void pick_config(int M, int N, int K, int sms, int* bn_out, int* cluster_out) {
   const int tiles_m = (M + BM - 1) / BM;
   const int num_kb = (K + BK - 1) / BK;
@@ -38,8 +44,8 @@ static void pick_config(int M, int N, int K, int sms, int* bn_out, int* cluster_
     const int units = ((tiles_m + c - 1) / c) * ((N + bn - 1) / bn);
     const int slots = sms / c;
     const int waves = (units + slots - 1) / slots;
-    const double per_kb = (c == 1) ? 0.1298 + 0.00184 * bn : 0.0602 + 0.00217 * bn;
-    const double per_tile = (c == 1) ? 0.3956 + 0.03142 * bn : 0.03538 * bn;
+    const double per_kb = (c == 1) ? 0.07216 + 0.00234 * bn : 0.00288 * bn;
+    const double per_tile = (c == 1) ? 0.12773 + 0.01752 * bn : 0.02067 * bn;
     const double cost = static_cast<double>(waves) * (num_kb * per_kb + per_tile);
     if (cost < best - 1e-9) { best = cost; *bn_out = bn; *cluster_out = c; }
   }

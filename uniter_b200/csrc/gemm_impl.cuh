@@ -2,15 +2,20 @@
 //
 //   D[M,N] = epilogue( sum_k A[m,k] * B[n,k] ),  16-bit operands, fp32 accumulation in registers.
 //
-// One persistent CTA per SM, three warpgroups with fixed roles:
+// One persistent CTA per SM, four warpgroups with fixed roles:
 //   warpgroup 0     TMA producer — one lane streams 128xBK A tiles and BNxBK B tiles into a
 //                   128B-swizzled smem ring (mbarrier full/empty pairs); the warpgroup gives
 //                   most of its registers to the consumers (setmaxnreg)
 //   warpgroups 1-2  consumers — each owns 64 rows of the 128 x BN tile: 4 x wgmma m64nBNk16 per
 //                   stage, a stage is released once the next stage's wgmma group is in flight;
-//                   then the epilogue from the accumulator registers: bias / dropout / residual /
-//                   GELU / dGELU / accumulate / column-sum, 16-byte stores
-// The producer runs ahead into the next tile while the consumers are in the epilogue.
+//                   then the finished accumulators go to shared memory, 64 columns at a time, into
+//                   a ring of EPI_CHUNKS fp32 chunks (mbarrier full/empty pairs), and the consumers
+//                   start the next tile's mainloop
+//   warpgroup 3     epilogue — drains each chunk: bias / dropout / residual / GELU / dGELU /
+//                   accumulate / column-sum, 16-byte stores
+// So the epilogue of one tile runs under the mainloop of the next: a 128-wide tile fits the ring
+// whole, wider tiles wait for the first chunks to drain.  The epilogue is the same fp32 code on the
+// same fp32 values as a register epilogue would run, so the output bits do not depend on the ring.
 //
 // kCluster = 2: a cluster of two CTAs on neighbouring 128-row tiles of the same BN columns.  Each
 // CTA loads its own A tile and HALF of the B tile, multicast into both CTAs, so every B tile is
@@ -31,7 +36,10 @@
 namespace ub {
 
 constexpr int A_TILE_BYTES = BM * BK * 2;
-constexpr int GEMM_THREADS = 384;       // producer warpgroup + 2 consumer warpgroups
+
+// Register-epilogue layout (gemm_ln.cu): producer + 2 consumer warpgroups, the consumers run the
+// epilogue from their accumulators through a per-warp 16 x 32 transpose buffer.
+constexpr int GEMM_THREADS = 384;
 constexpr int EPI_WARPS = 8;            // consumer warps, 16 accumulator rows each
 constexpr int EPI_PITCH = 33;           // fp32 words per row of a warp's 16 x 32 transpose buffer
 
@@ -43,6 +51,26 @@ struct GemmCfg {
   static constexpr int BAR_BYTES = 256;
   static constexpr int EPI_STAGE_BYTES = EPI_WARPS * 16 * EPI_PITCH * 4;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + EPI_STAGE_BYTES + 1024;  // + align slack
+};
+
+// Epilogue-warpgroup layout (gemm_kernel, gemm_group_kernel): the TMA ring, then the ring of fp32
+// hand-off chunks (128 rows x 64 columns each), then the mbarriers.  The chunks take the shared
+// memory of one TMA stage: 5 stages at BN = 128, 4 at 192, 3 at 256.
+constexpr int GEMM_WS_THREADS = 512;    // producer + 2 consumer + epilogue warpgroups
+constexpr int CHUNK_COLS = 64;
+constexpr int CHUNK_BYTES = BM * CHUNK_COLS * 4;
+constexpr int EPI_CHUNKS = 2;           // one whole 128-wide tile
+constexpr int MAX_DYN_SMEM = 227 * 1024;
+
+template <int BN>
+struct WsCfg {
+  static constexpr int STAGE_BYTES = GemmCfg<BN>::STAGE_BYTES;
+  static constexpr int RING_BYTES = EPI_CHUNKS * CHUNK_BYTES;
+  static constexpr int BAR_BYTES = 256;
+  static constexpr int FIT = (MAX_DYN_SMEM - RING_BYTES - BAR_BYTES - 1024) / STAGE_BYTES;
+  static constexpr int STAGES = FIT > 8 ? 8 : FIT;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + RING_BYTES + BAR_BYTES + 1024;  // + align slack
+  static_assert((2 * STAGES + 2 * EPI_CHUNKS) * 8 <= BAR_BYTES, "mbarriers overflow their region");
 };
 
 template <bool kBF16>
@@ -75,14 +103,11 @@ __device__ __forceinline__ void store8(void* base, long long idx, const float (&
 
 
 // --------------------------------------------------------------------------------- epilogue
-// One consumer warp: 16 accumulator rows [row0, row0 + 16) x BN columns from n0, in 32-column
-// blocks.  Accumulator register i of the wgmma fragment holds row (lane / 4) + 8 * ((i / 2) % 2),
-// column 8 * (i / 4) + 2 * (lane % 4) + i % 2.
+// Accumulator register i of the wgmma fragment holds row (lane / 4) + 8 * ((i / 2) % 2) of the
+// warp's 16 rows, column 8 * (i / 4) + 2 * (lane % 4) + i % 2.
 //
-//   * EPI >= 0 is a compile-time epilogue mask (the combinations the encoder uses are
-//     instantiated; EPI < 0 falls back to the runtime mask in p.epilogue);
-//   * side inputs of a block (bias / residual / dGELU aux / accumulate) are requested before the
-//     block is staged.
+// EPI >= 0 is a compile-time epilogue mask (the combinations the encoder uses are instantiated;
+// EPI < 0 falls back to the runtime mask in p.epilogue).
 template <int EPI, bool kBF16>
 struct EpiMask {
   const int rt;
@@ -94,11 +119,9 @@ struct EpiMask {
   }
 };
 
-// The fragment scatters a row over 4 lanes in 2-column pieces; storing (or loading side inputs)
-// in that mapping makes every warp-level access touch 8 rows in 8-byte pieces.  Each 16 x 32 block
-// therefore goes through a per-warp smem transpose (pitch 33 words) after which 4 lanes own one
-// row: every global access of the warp covers 8 rows x 64 contiguous bytes and the column sum
-// needs 3 shuffle steps.
+// Register-epilogue transpose (gemm_ln.cu): the fragment scatters a row over 4 lanes in 2-column
+// pieces, so each 16 x 32 block of a warp goes through smem (pitch 33 words), after which 4 lanes
+// own one row.
 template <int BN>
 __device__ __forceinline__ void stage_block(const float (&acc)[BN / 2], int c, int lane, float* stage) {
 #pragma unroll
@@ -109,58 +132,104 @@ __device__ __forceinline__ void stage_block(const float (&acc)[BN / 2], int c, i
   }
 }
 
-template <int EPI, int BN, bool kBF16>
-__device__ __forceinline__ void epilogue_warp(const GemmParams& p, const float (&acc)[BN / 2], int row0, int n0,
-                                              int lane, const DropoutRng& rng, float* stage) {
+// Word of element (r, c) in a 128 x 64 fp32 hand-off chunk.  Rows are 64 words; the 16-byte column
+// groups are XOR-swizzled by (r & 3) << 1 | (r & 1), so that the consumers' fragment writes (a
+// half-warp stores 8-byte pieces of 4 rows) and the epilogue's reads (a quarter-warp loads 16-byte
+// pieces of 2 rows) are both free of bank conflicts.
+__device__ __forceinline__ int chunk_word(int r, int c) {
+  return r * CHUNK_COLS + ((((c >> 2) ^ (((r & 3) << 1) | (r & 1)))) << 2) + (c & 3);
+}
+
+// Consumer warp: columns [64 c, 64 c + 64) of its 16 accumulator rows [r0, r0 + 16) into `chunk`.
+template <int BN>
+__device__ __forceinline__ void stage_chunk(const float (&acc)[BN / 2], int c, int r0, int lane, float* chunk) {
+#pragma unroll
+  for (int t = 0; t < 32; t += 2) {
+    const int r = r0 + (lane >> 2) + 8 * ((t >> 1) & 1);
+    const int cc = 8 * (t >> 2) + 2 * (lane & 3);
+    *reinterpret_cast<float2*>(chunk + chunk_word(r, cc)) = make_float2(acc[32 * c + t], acc[32 * c + t + 1]);
+  }
+}
+
+// Consumer warp `cw` (0..7): hand the finished tile to the epilogue warpgroup, one chunk per 64
+// columns (columns at or beyond N are never written, and no chunk is sent for them).
+template <int BN>
+__device__ __forceinline__ void handoff_tile(const float (&acc)[BN / 2], int n0, int N, int cw, int lane, float* ring,
+                                             uint64_t* chunk_full, uint64_t* chunk_empty, int& cs, uint32_t& cphase) {
+#pragma unroll
+  for (int c = 0; c < BN / CHUNK_COLS; ++c) {
+    if (n0 + c * CHUNK_COLS >= N) break;
+    mbar_wait(&chunk_empty[cs], cphase ^ 1);
+    stage_chunk<BN>(acc, c, 16 * cw, lane, ring + cs * (CHUNK_BYTES / 4));
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&chunk_full[cs]);
+    if (++cs == EPI_CHUNKS) { cs = 0; cphase ^= 1; }
+  }
+}
+
+// Epilogue warp `ew` (0..3): rows [m0 + 32 ew, m0 + 32 ew + 32) x columns [c0, c0 + 64) of the tile,
+// read from `chunk` once `full` completes its phase `parity`.  4 lanes own one row in 8-column
+// pieces: every global access of the warp covers 8 rows x 64 contiguous bytes and the column sum
+// needs 3 shuffle steps.  The side inputs (bias / residual / dGELU aux / accumulate) of the chunk
+// are requested before it is waited for.
+template <int EPI, bool kBF16>
+__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, int m0, int c0, int ew, int lane,
+                                               const DropoutRng& rng, const float* chunk, uint64_t* full,
+                                               uint32_t parity) {
   using T16 = typename Elem<kBF16>::T;
   const EpiMask<EPI, kBF16> E(p.epilogue);
   const int sub_r = lane >> 2;        // row inside an 8-row group
-  const int cg = (lane & 3) * 8;      // first of this lane's 8 columns inside the 32-column block
+  const int cg = (lane & 3) * 8;      // first of this lane's 8 columns inside a 32-column block
   const bool side16 = E.has(UB200_EPI_RESIDUAL) || E.has(UB200_EPI_DGELU) ||
                       (E.has(UB200_EPI_ACCUM) && !E.has(UB200_EPI_OUT_F32));
   const T16* side_base = E.has(UB200_EPI_RESIDUAL) ? reinterpret_cast<const T16*>(p.residual)
                          : (E.has(UB200_EPI_DGELU) ? reinterpret_cast<const T16*>(p.aux)
                                                    : reinterpret_cast<const T16*>(p.out));
   const long long side_ld = E.has(UB200_EPI_RESIDUAL) ? p.ldr : (E.has(UB200_EPI_DGELU) ? p.ldaux : p.ldo);
+  uint4 bias4[2], side[2][4];
 #pragma unroll
-  for (int c = 0; c < BN / 32; ++c) {
-    const int col0 = n0 + c * 32;
-    if (col0 >= p.N) break;           // warp-uniform
-    const int col = col0 + cg;
-    const bool col_ok = col < p.N;    // N % 8 == 0 is enforced on the host
-    uint4 bias4 = make_uint4(0, 0, 0, 0);
-    uint4 side[2];
+  for (int b = 0; b < 2; ++b) {
+    const int col = c0 + 32 * b + cg;
+    bias4[b] = make_uint4(0, 0, 0, 0);
 #pragma unroll
-    for (int it = 0; it < 2; ++it) side[it] = make_uint4(0, 0, 0, 0);
-    if (col_ok) {
+    for (int it = 0; it < 4; ++it) side[b][it] = make_uint4(0, 0, 0, 0);
+    if (col < p.N) {                  // N % 8 == 0 is enforced on the host
       if (E.has(UB200_EPI_BIAS))
-        bias4 = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.bias) + col));
+        bias4[b] = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.bias) + col));
       if (side16) {
 #pragma unroll
-        for (int it = 0; it < 2; ++it) {
-          const int row = row0 + it * 8 + sub_r;
+        for (int it = 0; it < 4; ++it) {
+          const int row = m0 + 32 * ew + it * 8 + sub_r;
           if (row < p.M)
-            side[it] = __ldg(reinterpret_cast<const uint4*>(side_base + static_cast<long long>(row) * side_ld + col));
+            side[b][it] = __ldg(reinterpret_cast<const uint4*>(side_base + static_cast<long long>(row) * side_ld + col));
         }
       }
     }
-    __syncwarp();                     // previous block's readers are done with `stage`
-    stage_block<BN>(acc, c, lane, stage);
-    __syncwarp();
+  }
+  mbar_wait(full, parity);
 
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    const int col0 = c0 + 32 * b;
+    if (col0 >= p.N) break;           // warp-uniform
+    const int col = col0 + cg;
+    const bool col_ok = col < p.N;
     float bias8[8];
-    unpack8_<kBF16>(bias4, bias8);
+    unpack8_<kBF16>(bias4[b], bias8);
     float csum[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) csum[i] = 0.f;
 
 #pragma unroll
-    for (int it = 0; it < 2; ++it) {
-      const int rr = it * 8 + sub_r;
-      const int row = row0 + rr;
+    for (int it = 0; it < 4; ++it) {
+      const int rr = 32 * ew + it * 8 + sub_r;
+      const int row = m0 + rr;
+      const float4 lo = *reinterpret_cast<const float4*>(chunk + chunk_word(rr, 32 * b + cg));
+      const float4 hi = *reinterpret_cast<const float4*>(chunk + chunk_word(rr, 32 * b + cg + 4));
+      const float a8[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
       float v[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = stage[rr * EPI_PITCH + cg + i] + bias8[i];
+      for (int i = 0; i < 8; ++i) v[i] = a8[i] + bias8[i];
       if (!(col_ok && row < p.M)) continue;
       if (E.has(UB200_EPI_DROPOUT)) {
         const uint64_t e = static_cast<uint64_t>(row) * static_cast<uint64_t>(p.N) + col;
@@ -170,7 +239,7 @@ __device__ __forceinline__ void epilogue_warp(const GemmParams& p, const float (
       }
       if (E.has(UB200_EPI_RESIDUAL)) {
         float t[8];
-        unpack8_<kBF16>(side[it], t);
+        unpack8_<kBF16>(side[b][it], t);
 #pragma unroll
         for (int i = 0; i < 8; ++i) v[i] += t[i];
       }
@@ -193,7 +262,7 @@ __device__ __forceinline__ void epilogue_warp(const GemmParams& p, const float (
         if (E.has(UB200_EPI_RESIDUAL))   // generic path only: aux was not prefetched
           load8<kBF16>(p.aux, static_cast<long long>(row) * p.ldaux + col, t);
         else
-          unpack8_<kBF16>(side[it], t);
+          unpack8_<kBF16>(side[b][it], t);
 #pragma unroll
         for (int i = 0; i < 8; ++i) v[i] *= dgelu_erf(t[i]);
       }
@@ -218,7 +287,7 @@ __device__ __forceinline__ void epilogue_warp(const GemmParams& p, const float (
           if (E.has(UB200_EPI_RESIDUAL) || E.has(UB200_EPI_DGELU))
             load8<kBF16>(p.out, static_cast<long long>(row) * p.ldo + col, t);   // generic path
           else
-            unpack8_<kBF16>(side[it], t);
+            unpack8_<kBF16>(side[b][it], t);
 #pragma unroll
           for (int i = 0; i < 8; ++i) v[i] += t[i];
         }
@@ -260,11 +329,22 @@ __device__ __forceinline__ void setmaxnreg_producer() {
 __device__ __forceinline__ void setmaxnreg_consumer() {
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
 }
+// 512-thread kernels start at 128 registers a thread: 24 + 2 x 192 + 104 = 4 x 128
+__device__ __forceinline__ void setmaxnreg_ws_producer() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
+}
+__device__ __forceinline__ void setmaxnreg_ws_consumer() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 192;" ::: "memory");
+}
+__device__ __forceinline__ void setmaxnreg_ws_epilogue() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 104;" ::: "memory");
+}
 
 // ------------------------------------------------------------------------------ pipeline halves
 // Producer lane: k-blocks [kb0, kb1) of the 128 x BN tile at (m0, n0) into the ring.  With
-// kCluster = 2 this CTA (cluster rank `rank`) loads half of the B tile and multicasts it.
-template <int BN, bool A_MN, bool B_MN, int kCluster>
+// kCluster = 2 this CTA (cluster rank `rank`) loads half of the B tile and multicasts it.  The ring
+// has kStages stages.
+template <int BN, bool A_MN, bool B_MN, int kCluster, int kStages = GemmCfg<BN>::STAGES>
 __device__ __forceinline__ void produce_tile(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                              const CUtensorMap* tmA, const CUtensorMap* tmB, int m0, int n0,
                                              int kb0, int kb1, int& stage, uint32_t& phase, uint32_t rank) {
@@ -301,14 +381,16 @@ __device__ __forceinline__ void produce_tile(uint8_t* smem, uint64_t* full_bar, 
         }
       }
     }
-    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+    if (++stage == kStages) { stage = 0; phase ^= 1; }
   }
 }
 
 // Consumer warpgroup `wg` (rows [64 wg, 64 wg + 64) of the tile): acc = A B^T over nkb k-blocks.
 // K-major operands advance 16 elements = 32 B inside the swizzle row per k16 step; MN-major ones
 // advance 16 K-rows = 2048 B, their 64-wide M/N groups are one 8 KB box apart.
-template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster>
+// kHalves256: issue a 256-wide tile as two m64n128 wgmmas (the 512-thread kernels, see below).
+template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster, int kStages = GemmCfg<BN>::STAGES,
+          bool kHalves256 = false>
 __device__ __forceinline__ void consume_tile(float (&acc)[BN / 2], uint8_t* smem, uint64_t* full_bar,
                                              uint64_t* empty_bar, int nkb, int wg, int& stage,
                                              uint32_t& phase, uint32_t peer) {
@@ -323,9 +405,21 @@ __device__ __forceinline__ void consume_tile(float (&acc)[BN / 2], uint8_t* smem
     const uint32_t sB = smem_u32(smem + stage * Cfg::STAGE_BYTES) + A_TILE_BYTES;
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < BK / 16; ++k)
-      Wgmma<BN, kBF16, A_MN, B_MN>::ss(acc, gmma_desc(sA + k * A_KSTEP, A_LBO, 1024),
-                                       gmma_desc(sB + k * B_KSTEP, B_LBO, 1024), (kb | k) != 0 ? 1u : 0u);
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t da = gmma_desc(sA + k * A_KSTEP, A_LBO, 1024);
+      const uint32_t scale_d = (kb | k) != 0 ? 1u : 0u;
+      if constexpr (BN == 256 && kHalves256) {
+        // two m64n128 halves (columns 128.. start 16 KB into the B tile, K- or MN-major): an m64n256
+        // wgmma needs more than the 128 registers a thread of a 512-thread kernel launches with.
+        // The fragment layout, and every output bit, is that of the m64n256 form.
+        float (&lo)[64] = *reinterpret_cast<float(*)[64]>(&acc[0]);
+        float (&hi)[64] = *reinterpret_cast<float(*)[64]>(&acc[64]);
+        Wgmma<128, kBF16, A_MN, B_MN>::ss(lo, da, gmma_desc(sB + k * B_KSTEP, B_LBO, 1024), scale_d);
+        Wgmma<128, kBF16, A_MN, B_MN>::ss(hi, da, gmma_desc(sB + 128 * 128 + k * B_KSTEP, B_LBO, 1024), scale_d);
+      } else {
+        Wgmma<BN, kBF16, A_MN, B_MN>::ss(acc, da, gmma_desc(sB + k * B_KSTEP, B_LBO, 1024), scale_d);
+      }
+    }
     wgmma_commit();
     wgmma_wait<1>();                   // the previous stage's wgmma group has retired
     if (prev >= 0 && releaser) {
@@ -333,7 +427,7 @@ __device__ __forceinline__ void consume_tile(float (&acc)[BN / 2], uint8_t* smem
       if (kCluster == 2) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[prev]), peer));
     }
     prev = stage;
-    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+    if (++stage == kStages) { stage = 0; phase ^= 1; }
   }
   wgmma_wait<0>();
   if (releaser) {
@@ -342,19 +436,60 @@ __device__ __forceinline__ void consume_tile(float (&acc)[BN / 2], uint8_t* smem
   }
 }
 
+// ============================================================ epilogue-warpgroup kernels: layout
+// WsCfg's carve-up of the (1024-aligned) dynamic shared memory.  Thread 0 initialises the barriers:
+// a TMA stage is emptied by the consumer warpgroups (of both CTAs with kCluster = 2), a chunk is
+// filled by the 8 consumer warps and emptied by the 4 epilogue warps.
+template <int BN>
+struct WsSmem {
+  using Cfg = WsCfg<BN>;
+  float* ring;
+  uint64_t* full_bar;
+  uint64_t* empty_bar;
+  uint64_t* chunk_full;
+  uint64_t* chunk_empty;
+  __device__ __forceinline__ explicit WsSmem(uint8_t* smem)
+      : ring(reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES)),
+        full_bar(reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::RING_BYTES)),
+        empty_bar(full_bar + Cfg::STAGES),
+        chunk_full(empty_bar + Cfg::STAGES),
+        chunk_empty(chunk_full + EPI_CHUNKS) {}
+  __device__ __forceinline__ void init(int kCluster) const {
+    for (int s = 0; s < Cfg::STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2 * kCluster);
+    }
+    for (int s = 0; s < EPI_CHUNKS; ++s) {
+      mbar_init(&chunk_full[s], EPI_WARPS);
+      mbar_init(&chunk_empty[s], 4);
+    }
+    fence_barrier_init();
+  }
+  // epilogue warp `ew`: the chunks of the tile at (m0, n0), in the order handoff_tile sends them
+  template <int EPI, bool kBF16>
+  __device__ __forceinline__ void drain_tile(const GemmParams& p, int m0, int n0, int ew, int lane,
+                                             const DropoutRng& rng, int& cs, uint32_t& cphase) const {
+    for (int c0 = n0; c0 < n0 + BN && c0 < p.N; c0 += CHUNK_COLS) {
+      epilogue_chunk<EPI, kBF16>(p, m0, c0, ew, lane, rng, ring + cs * (CHUNK_BYTES / 4), &chunk_full[cs], cphase);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&chunk_empty[cs]);
+      if (++cs == EPI_CHUNKS) { cs = 0; cphase ^= 1; }
+    }
+  }
+};
+
 // =================================================================================== GEMM kernel
 template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(GEMM_WS_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const GemmParams p) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = WsCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.  The offset is computed in the shared window
   // and applied by pointer arithmetic on the __shared__ array so that the compiler keeps the
   // shared address space (STS / LDS instead of generic ST / LD).
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
+  const WsSmem<BN> sm(smem);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -371,11 +506,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2 * kCluster);   // one arrive per consumer warpgroup (of both CTAs)
-    }
-    fence_barrier_init();
+    sm.init(kCluster);
   }
   pdl_launch_dependents();   // dependents may start their own prologue
   __syncthreads();
@@ -383,7 +514,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   pdl_wait();                // the producing kernel has completed; its outputs are visible
 
   if (warp < 4) {
-    setmaxnreg_producer();
+    setmaxnreg_ws_producer();
     // ===================================================================== TMA producer
     if (warp == 0 && lane == 0) {
       int stage = 0;
@@ -394,32 +525,40 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int kb1 = min(num_kb, kb0 + p.kb_per_split);
         const int m0 = (tile / p.tiles_n) * (kCluster * BM) + static_cast<int>(rank) * BM;
         const int n0 = (tile % p.tiles_n) * BN;
-        produce_tile<BN, A_MN, B_MN, kCluster>(smem, full_bar, empty_bar, &tmA, &tmB, m0, n0, kb0, kb1,
-                                               stage, phase, rank);
+        produce_tile<BN, A_MN, B_MN, kCluster, Cfg::STAGES>(smem, sm.full_bar, sm.empty_bar, &tmA, &tmB, m0, n0,
+                                                            kb0, kb1, stage, phase, rank);
       }
     }
-  } else {
-    setmaxnreg_consumer();
-    // ===================================================================== consumers + epilogue
-    const int cw = warp - 4;              // consumer warp 0..7
-    const int wg = cw >> 2;
-    const DropoutRng rng = make_rng(p);
-    float* epi_stage = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES) +
-                       cw * (16 * EPI_PITCH);
+  } else if (warp < 12) {
+    setmaxnreg_ws_consumer();
+    // ===================================================================== consumers
+    const int cw = warp - 4;              // consumer warp 0..7: tile rows [16 cw, 16 cw + 16)
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
+    int stage = 0, cs = 0;
+    uint32_t phase = 0, cphase = 0;
     for (int unit = unit0; unit < num_units; unit += unit_step) {
       const int tile = unit % num_tiles;
       const int kb0 = (unit / num_tiles) * p.kb_per_split;
       const int kb1 = min(num_kb, kb0 + p.kb_per_split);
+      const int n0 = (tile % p.tiles_n) * BN;
+      consume_tile<BN, A_MN, B_MN, kBF16, kCluster, Cfg::STAGES, true>(acc, smem, sm.full_bar, sm.empty_bar,
+                                                                       kb1 - kb0, cw >> 2, stage, phase, rank ^ 1u);
+      handoff_tile<BN>(acc, n0, p.N, cw, lane, sm.ring, sm.chunk_full, sm.chunk_empty, cs, cphase);
+    }
+  } else {
+    setmaxnreg_ws_epilogue();
+    // ===================================================================== epilogue
+    const int ew = warp - 12;             // epilogue warp 0..3: tile rows [32 ew, 32 ew + 32)
+    const DropoutRng rng = make_rng(p);
+    int cs = 0;
+    uint32_t cphase = 0;
+    for (int unit = unit0; unit < num_units; unit += unit_step) {
+      const int tile = unit % num_tiles;
       const int m0 = (tile / p.tiles_n) * (kCluster * BM) + static_cast<int>(rank) * BM;
       const int n0 = (tile % p.tiles_n) * BN;
-      consume_tile<BN, A_MN, B_MN, kBF16, kCluster>(acc, smem, full_bar, empty_bar, kb1 - kb0, wg, stage,
-                                                    phase, rank ^ 1u);
-      epilogue_warp<EPI, BN, kBF16>(p, acc, m0 + 16 * cw, n0, lane, rng, epi_stage);
+      sm.template drain_tile<EPI, kBF16>(p, m0, n0, ew, lane, rng, cs, cphase);
     }
   }
   if (kCluster == 2) cluster_sync_all();   // nobody exits while the peer may still signal it
@@ -443,32 +582,25 @@ __device__ __forceinline__ int group_of_tile(const GroupedParams& g, int tile) {
 }
 
 template <int BN, bool kBF16, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+__global__ void __launch_bounds__(GEMM_WS_THREADS, 1)
 gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = WsCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
+  const WsSmem<BN> sm(smem);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_kb = (g.K + BK - 1) / BK;
   const int num_tiles = g.tile_start[g.nprob];
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);
-    }
-    fence_barrier_init();
-  }
+  if (warp == 0 && lane == 0) sm.init(1);
   pdl_launch_dependents();
   __syncthreads();
   pdl_wait();
 
   if (warp < 4) {
-    setmaxnreg_producer();
+    setmaxnreg_ws_producer();
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -477,23 +609,33 @@ gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
         const int lt = tile - g.tile_start[pi];
         const int m0 = (lt / g.tiles_n[pi]) * BM;
         const int n0 = (lt % g.tiles_n[pi]) * BN;
-        produce_tile<BN, true, true, 1>(smem, full_bar, empty_bar, &tm.a[pi], &tm.b[pi], m0, n0, 0, num_kb,
-                                        stage, phase, 0u);
+        produce_tile<BN, true, true, 1, Cfg::STAGES>(smem, sm.full_bar, sm.empty_bar, &tm.a[pi], &tm.b[pi], m0, n0,
+                                                     0, num_kb, stage, phase, 0u);
       }
     }
-  } else {
-    setmaxnreg_consumer();
+  } else if (warp < 12) {
+    setmaxnreg_ws_consumer();
     const int cw = warp - 4;
-    const int wg = cw >> 2;
-    DropoutRng rng;
-    rng.k0 = rng.k1 = rng.s0 = rng.s1 = 0; rng.thr16 = 0; rng.inv_keep = 1.f;
-    float* epi_stage = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES) +
-                       cw * (16 * EPI_PITCH);
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
+    int stage = 0, cs = 0;
+    uint32_t phase = 0, cphase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int pi = group_of_tile(g, tile);
+      const int lt = tile - g.tile_start[pi];
+      const int n0 = (lt % g.tiles_n[pi]) * BN;
+      consume_tile<BN, true, true, kBF16, 1, Cfg::STAGES, true>(acc, smem, sm.full_bar, sm.empty_bar, num_kb,
+                                                                cw >> 2, stage, phase, 0u);
+      handoff_tile<BN>(acc, n0, g.N[pi], cw, lane, sm.ring, sm.chunk_full, sm.chunk_empty, cs, cphase);
+    }
+  } else {
+    setmaxnreg_ws_epilogue();
+    const int ew = warp - 12;
+    DropoutRng rng;
+    rng.k0 = rng.k1 = rng.s0 = rng.s1 = 0; rng.thr16 = 0; rng.inv_keep = 1.f;
+    int cs = 0;
+    uint32_t cphase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int pi = group_of_tile(g, tile);
       const int lt = tile - g.tile_start[pi];
@@ -502,8 +644,7 @@ gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
       GemmParams pp{};
       pp.M = g.M[pi]; pp.N = g.N[pi]; pp.K = g.K; pp.epilogue = g.epilogue;
       pp.out = g.out[pi]; pp.ldo = g.ldo[pi];
-      consume_tile<BN, true, true, kBF16, 1>(acc, smem, full_bar, empty_bar, num_kb, wg, stage, phase, 0u);
-      epilogue_warp<EPI, BN, kBF16>(pp, acc, m0 + 16 * cw, n0, lane, rng, epi_stage);
+      sm.template drain_tile<EPI, kBF16>(pp, m0, n0, ew, lane, rng, cs, cphase);
     }
   }
 }
@@ -511,7 +652,7 @@ gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
 template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster, int EPI>
 static int launch_gemm(const GemmParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, int grid,
                        cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = WsCfg<BN>;
   void (*kern)(const CUtensorMap, const CUtensorMap, const GemmParams) = gemm_kernel<BN, A_MN, B_MN, kBF16, kCluster, EPI>;
   static unsigned long long configured = 0;  // per instantiation, one bit per device
   if (first_use_on_device(configured))
@@ -519,7 +660,7 @@ static int launch_gemm(const GemmParams& p, const CUtensorMap& tmA, const CUtens
                                        Cfg::SMEM_BYTES));
   {
     ProfScope ps(stream);
-    UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, kCluster,
+    UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(GEMM_WS_THREADS), Cfg::SMEM_BYTES, stream, kCluster,
                              tmA, tmB, p));
   }
   return 0;
@@ -582,7 +723,7 @@ int gemm_dispatch(int bn, int cluster, int a_major, int b_major, const GemmParam
 
 template <int BN, bool kBF16>
 int gemm_group_launch(const TmPack& tm, const GroupedParams& g, int grid, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = WsCfg<BN>;
   void (*kern)(const TmPack, const GroupedParams);
   if (g.epilogue == 0) kern = gemm_group_kernel<BN, kBF16, 0>;
   else if (g.epilogue == UB200_EPI_ACCUM) kern = gemm_group_kernel<BN, kBF16, UB200_EPI_ACCUM>;
@@ -592,7 +733,7 @@ int gemm_group_launch(const TmPack& tm, const GroupedParams& g, int grid, cudaSt
   if (first_use_on_device(configured[ci]))
     UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   ProfScope ps(stream);
-  UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, 1, tm, g));
+  UB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(GEMM_WS_THREADS), Cfg::SMEM_BYTES, stream, 1, tm, g));
   return 0;
 }
 
