@@ -33,7 +33,11 @@ def gelu_erf(x):
 
 def layer_norm(x, weight, bias, eps=1e-12):
     """apex FusedLayerNorm as used at model/layer.py:108,149 and model/model.py:228,254-259:
-    mean / biased variance over the last dim, eps added inside the sqrt, affine."""
+    mean / biased variance over the last dim, eps added inside the sqrt, affine.  16-bit inputs keep
+    fp32 statistics and round once, as apex does for half inputs (torch's native layer_norm has the
+    same contract)."""
+    if x.dtype in (torch.float16, torch.bfloat16):
+        return torch.nn.functional.layer_norm(x, (x.size(-1),), weight, bias, eps)
     mu = x.mean(-1, keepdim=True)
     var = ((x - mu) ** 2).mean(-1, keepdim=True)
     return (x - mu) / torch.sqrt(var + eps) * weight + bias
@@ -44,22 +48,38 @@ def linear(x, w, b=None):
     return y if b is None else y + b
 
 
+def dropout(x, keep=None, inv_keep=1.0):
+    """nn.Dropout with a given keep mask (bool, broadcasting against x): x * keep * inv_keep, computed
+    in at least fp32 and rounded once to x's dtype as torch's dropout does; identity without a mask."""
+    if keep is None:
+        return x
+    w = torch.promote_types(x.dtype, torch.float32)
+    return (x.to(w) * (keep.to(w) * inv_keep)).to(x.dtype)
+
+
 # ----------------------------------------------------------------------------- embeddings
-def text_embeddings(state, input_ids, position_ids, token_type_ids=None, prefix="embeddings."):
-    """model/model.py:232-245 — LN(word[ids] + pos[position_ids] + type[tt]); dropout omitted
-    (oracle runs at p=0).  position_ids is [1, Lt] and broadcasts over the batch."""
+def text_embeddings(state, input_ids, position_ids, token_type_ids=None, prefix="embeddings.",
+                    keep=None, inv_keep=1.0, taps=None):
+    """model/model.py:232-245 — dropout(LN(word[ids] + pos[position_ids] + type[tt])), the dropout
+    given as a keep mask (none: p = 0).  position_ids is [1, Lt] and broadcasts over the batch.
+    taps["u"]: the sum before the LayerNorm."""
     if token_type_ids is None:
         token_type_ids = torch.zeros_like(input_ids)
     e = (state[prefix + "word_embeddings.weight"][input_ids]
          + state[prefix + "position_embeddings.weight"][position_ids]
          + state[prefix + "token_type_embeddings.weight"][token_type_ids])
-    return layer_norm(e, state[prefix + "LayerNorm.weight"], state[prefix + "LayerNorm.bias"])
+    if taps is not None:
+        taps["u"] = e
+    return dropout(layer_norm(e, state[prefix + "LayerNorm.weight"], state[prefix + "LayerNorm.bias"]),
+                   keep, inv_keep)
 
 
 def image_embeddings(state, img_feat, img_pos_feat, img_type_ids=None, img_masks=None,
-                     prefix="img_embeddings."):
-    """model/model.py:311-319 + :261-272 — LN( LN(img_linear(f)) + LN(pos_linear(p)) + type ).
-    With img_masks, row 1 of mask_embedding is added to masked regions (row 0 is forced to 0)."""
+                     prefix="img_embeddings.", keep=None, inv_keep=1.0, taps=None):
+    """model/model.py:311-319 + :261-272 — dropout(LN( LN(img_linear(f)) + LN(pos_linear(p)) + type )),
+    the dropout given as a keep mask (none: p = 0).  With img_masks, row 1 of mask_embedding is added
+    to masked regions (row 0 is forced to 0).  taps["u"]: the sum before the last LayerNorm,
+    taps["ppre"]: the pos_linear output."""
     if img_type_ids is None:
         img_type_ids = torch.ones(img_feat.shape[:2], dtype=torch.long)
     type_emb = state["embeddings.token_type_embeddings.weight"][img_type_ids]
@@ -70,11 +90,13 @@ def image_embeddings(state, img_feat, img_pos_feat, img_type_ids=None, img_masks
     t_im = layer_norm(linear(img_feat, state[prefix + "img_linear.weight"],
                              state[prefix + "img_linear.bias"]),
                       state[prefix + "img_layer_norm.weight"], state[prefix + "img_layer_norm.bias"])
-    t_pos = layer_norm(linear(img_pos_feat, state[prefix + "pos_linear.weight"],
-                              state[prefix + "pos_linear.bias"]),
-                       state[prefix + "pos_layer_norm.weight"], state[prefix + "pos_layer_norm.bias"])
-    return layer_norm(t_im + t_pos + type_emb, state[prefix + "LayerNorm.weight"],
-                      state[prefix + "LayerNorm.bias"])
+    ppre = linear(img_pos_feat, state[prefix + "pos_linear.weight"], state[prefix + "pos_linear.bias"])
+    t_pos = layer_norm(ppre, state[prefix + "pos_layer_norm.weight"], state[prefix + "pos_layer_norm.bias"])
+    u = t_im + t_pos + type_emb
+    if taps is not None:
+        taps["u"], taps["ppre"] = u, ppre
+    return dropout(layer_norm(u, state[prefix + "LayerNorm.weight"], state[prefix + "LayerNorm.bias"]),
+                   keep, inv_keep)
 
 
 def gather_embeddings(txt_emb, img_emb, gather_index):

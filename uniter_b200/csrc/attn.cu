@@ -1035,11 +1035,9 @@ static AttnParams attn_params(const ub200_attn_args& a) {
   p.ctx = a.ctx; p.lse = a.lse;
   p.scale = 0.125f;
   if (a.dropout_p > 0.f) {
-    uint32_t thr = static_cast<uint32_t>(a.dropout_p * 65536.0f + 0.5f);
-    if (thr > 65535u) thr = 65535u;
-    if (thr == 0u) thr = 1u;
-    p.drop_thr16 = thr;
-    p.drop_inv_keep = 65536.0f / static_cast<float>(65536u - thr);
+    const DropoutThreshold d = dropout_threshold(a.dropout_p);
+    p.drop_thr16 = d.thr16;
+    p.drop_inv_keep = d.inv_keep;
   } else {
     p.drop_thr16 = 0; p.drop_inv_keep = 1.f;
   }

@@ -23,6 +23,21 @@ int set_error(int code, const char* fmt, ...);  // stores message, returns code
                              __FILE__, __LINE__);                                             \
   } while (0)
 
+// Dropout threshold of every dropout site for drop probability p in (0, 1): an element is dropped iff
+// its 16-bit Philox value is below thr16, and kept values are scaled by inv_keep.  thr16 is clamped to
+// [1, 65535], so a forward and a backward that both derive it from the same p agree on the mask for
+// every p > 0, however small (oracle/philox.py dropout_params is the host mirror).
+struct DropoutThreshold {
+  uint32_t thr16;
+  float inv_keep;
+};
+inline DropoutThreshold dropout_threshold(float p) {
+  uint32_t thr = static_cast<uint32_t>(p * 65536.0f + 0.5f);
+  if (thr > 65535u) thr = 65535u;
+  if (thr == 0u) thr = 1u;
+  return {thr, 65536.0f / static_cast<float>(65536u - thr)};
+}
+
 int num_sms();  // SM count of the current device (cached)
 int deterministic();  // ub200_set_deterministic: launches use fixed-order reductions, no float atomics
 

@@ -600,10 +600,8 @@ extern "C" int ub200_embed_rows_fwd(const ub200_embed_rows_args* a, ub200_stream
   p.ln_f_g = a->ln_out_g; p.ln_f_b = a->ln_out_b;
   p.x = a->x; p.u = a->u; p.ppre = a->ppre; p.T = a->T; p.H = a->hidden;
   if (a->dropout_p > 0.f) {
-    uint32_t thr = static_cast<uint32_t>(a->dropout_p * 65536.0f + 0.5f);
-    if (thr > 65535u) thr = 65535u;
-    if (thr == 0u) thr = 1u;
-    p.drop_thr16 = thr; p.drop_inv_keep = 65536.0f / static_cast<float>(65536u - thr);
+    const DropoutThreshold d = dropout_threshold(a->dropout_p);
+    p.drop_thr16 = d.thr16; p.drop_inv_keep = d.inv_keep;
   } else {
     p.drop_thr16 = 0; p.drop_inv_keep = 1.f;
   }

@@ -124,10 +124,9 @@ extern "C" int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream_) {
     p.bias = a.bias; p.residual = a.residual; p.out = a.out;
     p.ldr = a.ldr; p.ldo = a.ldo;
     if ((epi & UB200_EPI_DROPOUT) && a.dropout_p > 0.f) {
-      uint32_t thr = static_cast<uint32_t>(a.dropout_p * 65536.0f + 0.5f);
-      if (thr > 65535u) thr = 65535u;
-      p.drop_thr16 = thr;
-      p.drop_inv_keep = 65536.0f / static_cast<float>(65536u - thr);
+      const DropoutThreshold d = dropout_threshold(a.dropout_p);
+      p.drop_thr16 = d.thr16;
+      p.drop_inv_keep = d.inv_keep;
     } else {
       p.epilogue &= ~UB200_EPI_DROPOUT;
       p.drop_thr16 = 0;
@@ -182,10 +181,9 @@ extern "C" int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream_) {
   p.out = a.out; p.out2 = a.out2; p.colsum = a.colsum;
   p.ldr = a.ldr; p.ldaux = a.ldaux; p.ldo = a.ldo;
   if ((epi & UB200_EPI_DROPOUT) && a.dropout_p > 0.f) {
-    uint32_t thr = static_cast<uint32_t>(a.dropout_p * 65536.0f + 0.5f);
-    if (thr > 65535u) thr = 65535u;
-    p.drop_thr16 = thr;
-    p.drop_inv_keep = 65536.0f / static_cast<float>(65536u - thr);
+    const DropoutThreshold d = dropout_threshold(a.dropout_p);
+    p.drop_thr16 = d.thr16;
+    p.drop_inv_keep = d.inv_keep;
   } else {
     p.epilogue &= ~UB200_EPI_DROPOUT;
     p.drop_thr16 = 0;

@@ -809,13 +809,11 @@ extern "C" int ub200_layernorm_bwd(const ub200_ln_bwd_args* a, ub200_stream_t st
   p.zero_inactive = (a->dropout_on_dy & 2) ? 1 : 0;
   if (a->dropout_p > 0.f) {
     UB_CHECK_ARG(a->dx_drop || (a->dropout_on_dy & 1), "layernorm_bwd: dropout_p > 0 needs dx_drop");
-    uint32_t thr = static_cast<uint32_t>(a->dropout_p * 65536.0f + 0.5f);
-    if (thr > 65535u) thr = 65535u;
-    if (thr == 0u) thr = 1u;
+    const ub::DropoutThreshold d = ub::dropout_threshold(a->dropout_p);
     p.dx_drop = (a->dropout_on_dy & 1) ? nullptr : a->dx_drop;
     p.dy_drop = (a->dropout_on_dy & 1) ? 1 : 0;
-    p.drop_thr16 = thr;
-    p.drop_inv_keep = 65536.0f / static_cast<float>(65536u - thr);
+    p.drop_thr16 = d.thr16;
+    p.drop_inv_keep = d.inv_keep;
   } else {
     p.dx_drop = nullptr; p.drop_thr16 = 0; p.drop_inv_keep = 1.f;
   }
