@@ -415,6 +415,51 @@ int ub200_dgelu_mul(const void* dy, const void* pre, void* out, int64_t n, int32
 int ub200_dtanh_mul(const void* dy, const void* y, void* out, int64_t n, int32_t dtype,
                     ub200_stream_t stream);
 
+/* Referring-expression head (model/re.py:48-100): one Linear(H, 1) score per image region and the
+ * per-sample loss over a sample's regions.  `rows` is a [R, H] 16-bit matrix of region rows (H % 8 ==
+ * 0, 16-byte aligned); sample b owns rows seg_start[b] .. seg_start[b] + seg_len[b] - 1 (int32 device
+ * tables).  Segments are disjoint and ascending; rows outside every segment are padding.  One CTA per
+ * sample.  Per sample b and region k < max_regions:
+ *   score[b, k] = round16(rows[seg_start[b] + k] . weight + bias)     (fp32 accumulation)
+ *   score[b, k] = round16(-1e4) where k >= seg_len[b] or obj_masks[b, k] != 0   (masked_fill)
+ * and, for targets t = targets[b] in [0, seg_len[b]) (others: loss 0, no gradient):
+ *   UB200_RE_CLS   loss[b] = logsumexp(score[b, :]) - score[b, t] in fp32; lse[b] saved
+ *   UB200_RE_RANK  loss[b] = max(margin + sigmoid(score[b, n]) - sigmoid(score[b, t]), 0), where
+ *                  n = neg_plan[b] if >= 0 (an easy negative drawn by the caller), and for
+ *                  neg_plan[b] == -1 the highest-scoring unmasked region != t (ties: lowest index);
+ *                  the chosen n is saved in neg_ix[b]
+ * The backward writes dscore = dloss * (softmax - onehot) (cls) or -+ sigmoid'(s) * dloss at t / n
+ * where the hinge is >= 0 (rank), 0 at masked positions;  d_rows[r] = round16(dscore * weight) for the
+ * rows of every segment and 0 for padding rows;  dweight[H] = sum dscore * rows and dbias[0] = sum
+ * dscore in fp32, written (not accumulated).  The two weight sums are per-sample partials (workspace)
+ * added in sample order by a second launch: no float atomics, the same bits in every mode. */
+enum { UB200_RE_SCORES = 0, UB200_RE_CLS = 1, UB200_RE_RANK = 2 };
+typedef struct {
+  const void* rows;          /* [R, H] */
+  const void* weight;        /* [H] */
+  const void* bias;          /* [1] or NULL */
+  const int32_t* seg_start;  /* [batch] */
+  const int32_t* seg_len;    /* [batch] */
+  const uint8_t* obj_masks;  /* [batch, max_regions], non-zero = masked (uint8 or bool) */
+  const int64_t* targets;    /* [batch] (cls / rank) */
+  const int64_t* neg_plan;   /* [batch] (rank) */
+  void* scores;              /* [batch, max_regions] 16-bit */
+  float* loss;               /* [batch] (cls / rank) */
+  float* lse;                /* [batch] (cls) */
+  int32_t* neg_ix;           /* [batch] (rank) */
+  const float* dloss;        /* [batch] (backward) */
+  void* d_rows;              /* [R, H] (backward) */
+  float* dweight;            /* [H] (backward) */
+  float* dbias;              /* [1] (backward) */
+  void* workspace;           /* >= ub200_region_score_workspace_bytes (backward) */
+  int64_t workspace_bytes;
+  int32_t R, hidden, batch, max_regions, mode, dtype;
+  float margin;
+} ub200_region_score_args;
+int64_t ub200_region_score_workspace_bytes(int32_t batch, int32_t hidden);
+int ub200_region_score_fwd(const ub200_region_score_args* args, ub200_stream_t stream);
+int ub200_region_score_bwd(const ub200_region_score_args* args, ub200_stream_t stream);
+
 /* Multi-tensor AdamW on fp32 master weights: replaces optim/adamw.py:43-103 (+ the apex O2
  * master-gradient copy, unscale and master->model copy around it, train_vqa.py:152,190-227) and
  * torch.nn.utils.clip_grad_norm_ (train_vqa.py:223-226).  One segment per parameter tensor;

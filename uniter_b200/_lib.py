@@ -116,6 +116,18 @@ class PeerAllreduceArgs(C.Structure):
                 ("timeout_ms", C.c_int32)]
 
 
+RE_SCORES, RE_CLS, RE_RANK = 0, 1, 2
+
+
+class RegionScoreArgs(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in (
+        "rows", "weight", "bias", "seg_start", "seg_len", "obj_masks", "targets", "neg_plan", "scores",
+        "loss", "lse", "neg_ix", "dloss", "d_rows", "dweight", "dbias", "workspace")] + [
+        ("workspace_bytes", C.c_int64),
+        ("R", C.c_int32), ("hidden", C.c_int32), ("batch", C.c_int32), ("max_regions", C.c_int32),
+        ("mode", C.c_int32), ("dtype", C.c_int32), ("margin", C.c_float)]
+
+
 F32 = 2
 _lib = None
 
@@ -203,6 +215,11 @@ def load():
     lib.ub200_adamw_step_scaled.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_float,
                                             C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_int32, C.c_void_p]
+    lib.ub200_region_score_workspace_bytes.restype = C.c_int64
+    lib.ub200_region_score_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
+    for name in ("ub200_region_score_fwd", "ub200_region_score_bwd"):
+        getattr(lib, name).restype = C.c_int
+        getattr(lib, name).argtypes = [C.POINTER(RegionScoreArgs), C.c_void_p]
     lib.ub200_gather_rows.restype = C.c_int
     lib.ub200_gather_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.ub200_peer_flags_bytes.restype = C.c_int64

@@ -11,6 +11,8 @@ GPU path run without a single device->host read:
   ``txt_lens``, ``num_bbs`` (python lists), ``cu_seqlens`` (int32 [B+1], packed-row offsets of each
   sample), and for MLM ``mlm_index`` / ``mlm_targets`` (flat b*L+j positions and labels of the
   masked tokens, in the order of the reference's boolean-mask selection, model/pretrain.py:129-133).
+* ``re_collate`` / ``re_eval_collate`` — data/re.py:146-188, :251-295, plus ``re_index`` / ``re_seg``, the
+  flat positions of the region rows and each sample's start and count in them (``re_region_index``).
 * ``DevicePrefetcher`` — data/loader.py:86-141 (side-stream H2D of pinned batches, joined with
   ``wait_stream`` + ``record_stream``), additionally registering the per-sample lengths of the
   device attention mask with the model (``register_lengths``) so forward() never syncs.
@@ -125,6 +127,56 @@ def mlm_collate(inputs):
     pos = (txt_labels != -1).nonzero(as_tuple=False)
     batch["mlm_index"] = (pos[:, 0] * L + pos[:, 1]).contiguous()
     batch["mlm_targets"] = txt_labels[pos[:, 0], pos[:, 1]].contiguous()
+    return batch
+
+
+def re_region_index(txt_lens, num_bbs, L, multiple=64):
+    """Where the image regions of a referring-expression batch sit (model/re.py:129-157,
+    `_get_image_hidden`): flat positions b * L + txt_lens[b] + k of the padded [B, L] layout, padded
+    with the "no row" position B * L to a multiple of `multiple` (int64), and int32 [2, B] with the
+    start of each sample's regions in that list and their count."""
+    B = len(txt_lens)
+    flat, starts = [], []
+    for b, (tl, nbb) in enumerate(zip(txt_lens, num_bbs)):
+        starts.append(len(flat))
+        flat.extend(range(b * L + tl, b * L + tl + nbb))
+    n = max((len(flat) + multiple - 1) // multiple * multiple, multiple)
+    flat.extend([B * L] * (n - len(flat)))
+    return torch.tensor(flat, dtype=torch.long), torch.tensor([starts, list(num_bbs)], dtype=torch.int32)
+
+
+def _re_fields(input_ids, img_feats, img_pos_feats, attn_masks, obj_masks):
+    """data/re.py:146-188 without the targets: the joint fields, obj_masks padded with 1 (uint8, as the
+    datasets build it), and the region index of re_region_index as `re_index` / `re_seg`."""
+    batch = _joint_fields(input_ids, img_feats, img_pos_feats, attn_masks)
+    if min(batch["num_bbs"]) < 1:
+        raise ValueError("every sample needs at least one region, got num_bbs %s" % batch["num_bbs"])
+    batch["obj_masks"] = pad_sequence(obj_masks, batch_first=True, padding_value=1)
+    batch["re_index"], batch["re_seg"] = re_region_index(batch["txt_lens"], batch["num_bbs"],
+                                                         batch["attn_masks"].size(1))
+    return batch
+
+
+def re_collate(inputs):
+    """inputs: list of (input_ids, img_feat, img_pos_feat, attn_masks, obj_masks [nbb] uint8, target [1])
+    — data/re.py:146-188 (ReDataset)."""
+    input_ids, img_feats, img_pos_feats, attn_masks, obj_masks, targets = map(list, zip(*inputs))
+    batch = _re_fields(input_ids, img_feats, img_pos_feats, attn_masks, obj_masks)
+    targets = torch.stack(targets, dim=0)
+    for t, nbb in zip(targets.view(-1).tolist(), batch["num_bbs"]):
+        if not 0 <= t < nbb:
+            raise ValueError("target %d outside [0, %d)" % (t, nbb))
+    batch["targets"] = targets
+    return batch
+
+
+def re_eval_collate(inputs):
+    """inputs: list of (input_ids, img_feat, img_pos_feat, attn_masks, obj_masks, tgt_box, obj_boxes,
+    sent_id) — data/re.py:251-295 (ReEvalDataset)."""
+    (input_ids, img_feats, img_pos_feats, attn_masks, obj_masks, tgt_box, obj_boxes,
+     sent_ids) = map(list, zip(*inputs))
+    batch = _re_fields(input_ids, img_feats, img_pos_feats, attn_masks, obj_masks)
+    batch["tgt_box"], batch["obj_boxes"], batch["sent_ids"] = tgt_box, obj_boxes, sent_ids
     return batch
 
 

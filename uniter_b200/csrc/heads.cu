@@ -12,6 +12,9 @@
 //                     AFTER the Adam update) on fp32 master weights, fused with gradient
 //                     unscaling, global-norm clipping (train_vqa.py:223-226) and the 16-bit
 //                     model-weight refresh that apex O2 does as separate passes.
+//   region_score      referring-expression head (model/re.py:69-90): Linear(H, 1) over each
+//                     sample's region rows, masked_fill, cross-entropy or ranking hinge, and the
+//                     backward with fixed-order weight-gradient sums (no float atomics).
 #include "common.h"
 #include "ptx.cuh"
 
@@ -360,6 +363,196 @@ adamw_kernel(const ub200_adam_segment* __restrict__ segs, const int* __restrict_
   }
 }
 
+// ------------------------------------------------------------------------------ referring expressions
+// model/re.py:69-90: re_output (Linear(H, 1)) over each sample's region rows, masked_fill(obj_masks,
+// -1e4), then CrossEntropyLoss or the sigmoid ranking hinge.  One CTA per sample (<= ~100 regions).
+constexpr int RE_THREADS = 256;
+constexpr int RE_MAX_REGIONS = 8192;   // scores of one sample in shared memory (32 KB)
+
+__device__ __forceinline__ float re_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+__device__ __forceinline__ bool re_live(const uint8_t* __restrict__ obj_masks, int b, int k, int len, int Smax) {
+  return k < len && obj_masks[static_cast<long long>(b) * Smax + k] == 0;
+}
+
+// The ranking hinge margin + sigmoid(s_n) - sigmoid(s_t), recomputed bit for bit by the backward.
+__device__ __forceinline__ float re_hinge(float margin, float s_neg, float s_pos) {
+  return margin + re_sigmoid(s_neg) - re_sigmoid(s_pos);
+}
+
+template <bool kBF16>
+__global__ void __launch_bounds__(RE_THREADS)
+region_score_fwd_kernel(const ub200_region_score_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  using T16 = typename Elem<kBF16>::T;
+  extern __shared__ float re_sc[];          // [Smax] rounded scores
+  __shared__ float red[8];
+  const int b = blockIdx.x, Smax = a.max_regions, H = a.hidden;
+  const int start = a.seg_start[b], len = a.seg_len[b];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint4* wv = reinterpret_cast<const uint4*>(a.weight);
+  const float bias = a.bias != nullptr ? Elem<kBF16>::to_f(*reinterpret_cast<const T16*>(a.bias)) : 0.f;
+  const float masked = Elem<kBF16>::to_f(Elem<kBF16>::from_f(-1e4f));
+  // one warp per region: lane-strided 16-byte vectors, fp32 FMA chains, then a fixed xor tree
+  for (int k = warp; k < Smax; k += RE_THREADS / 32) {
+    float s = masked;
+    if (re_live(a.obj_masks, b, k, len, Smax)) {
+      const uint4* hv = reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(a.rows) +
+                                                       static_cast<long long>(start + k) * H);
+      float acc = 0.f;
+      for (int v = lane; v < (H >> 3); v += 32) {
+        float h[8], w[8];
+        h_unpack8<kBF16>(__ldg(hv + v), h);
+        h_unpack8<kBF16>(__ldg(wv + v), w);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc = fmaf(h[e], w[e], acc);
+      }
+#pragma unroll
+      for (int o = 16; o >= 1; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+      s = Elem<kBF16>::to_f(Elem<kBF16>::from_f(acc + bias));
+    }
+    if (lane == 0) re_sc[k] = s;
+  }
+  __syncthreads();
+  T16* out = reinterpret_cast<T16*>(a.scores) + static_cast<long long>(b) * Smax;
+  for (int k = threadIdx.x; k < Smax; k += RE_THREADS) out[k] = Elem<kBF16>::from_f(re_sc[k]);
+  if (a.mode == UB200_RE_SCORES) return;
+  const long long t = a.targets[b];
+  const bool tvalid = t >= 0 && t < len;
+  if (a.mode == UB200_RE_CLS) {
+    // CrossEntropyLoss over the whole masked row: masked positions hold -1e4 and add exp(-1e4 - m) = 0
+    float m = -INFINITY;
+    for (int k = threadIdx.x; k < Smax; k += RE_THREADS) m = fmaxf(m, re_sc[k]);
+    m = block_max(m, red);
+    float s = 0.f;
+    for (int k = threadIdx.x; k < Smax; k += RE_THREADS) s += expf(re_sc[k] - m);
+    s = block_sum(s, red);
+    if (threadIdx.x == 0) {
+      const float lse = m + logf(s);
+      a.lse[b] = lse;
+      a.loss[b] = tvalid ? lse - re_sc[t] : 0.f;
+    }
+    return;
+  }
+  if (threadIdx.x != 0) return;
+  int n = -1;
+  if (tvalid) {
+    const long long p = a.neg_plan[b];
+    if (p >= 0) {
+      if (p < len && p != t) n = static_cast<int>(p);
+    } else {
+      // hard negative (model/re.py:115-121): the best region != t, unmasked ones first, ties to the
+      // lowest index; a sample whose other regions are all masked falls back to its lowest other index
+      bool best_live = false;
+      float best = 0.f;
+      for (int k = 0; k < len; ++k) {
+        if (k == t) continue;
+        const bool live = re_live(a.obj_masks, b, k, len, Smax);
+        if (n < 0 || (live && !best_live) || (live == best_live && re_sc[k] > best)) {
+          n = k;
+          best = re_sc[k];
+          best_live = live;
+        }
+      }
+    }
+  }
+  a.neg_ix[b] = n;
+  a.loss[b] = n >= 0 ? fmaxf(re_hinge(a.margin, re_sc[n], re_sc[t]), 0.f) : 0.f;
+}
+
+// dscore into shared memory, then per column vector: d_rows = dscore * w over the segment's rows and
+// the sample's partial of dweight (rows in ascending order); padding rows after the segment (and
+// before the first one) are zeroed by the CTA that owns the preceding segment.
+template <bool kBF16>
+__global__ void __launch_bounds__(RE_THREADS)
+region_score_bwd_kernel(const ub200_region_score_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  using T16 = typename Elem<kBF16>::T;
+  extern __shared__ float re_ds[];          // [Smax] dscore
+  const int b = blockIdx.x, Smax = a.max_regions, H = a.hidden;
+  const int start = a.seg_start[b], len = a.seg_len[b];
+  const T16* sc = reinterpret_cast<const T16*>(a.scores) + static_cast<long long>(b) * Smax;
+  const long long t = a.targets[b];
+  const bool tvalid = t >= 0 && t < len;
+  const float g = a.dloss[b];
+  float* part_w = reinterpret_cast<float*>(a.workspace);
+  float* part_b = part_w + static_cast<long long>(a.batch) * H;
+  const float lse = a.mode == UB200_RE_CLS ? a.lse[b] : 0.f;
+  for (int k = threadIdx.x; k < Smax; k += RE_THREADS) {
+    float d = 0.f;
+    if (a.mode == UB200_RE_CLS && tvalid && re_live(a.obj_masks, b, k, len, Smax))
+      d = (expf(Elem<kBF16>::to_f(sc[k]) - lse) - (k == t ? 1.f : 0.f)) * g;
+    re_ds[k] = d;
+  }
+  __syncthreads();
+  if (a.mode == UB200_RE_RANK && threadIdx.x == 0) {
+    const int n = a.neg_ix[b];
+    if (tvalid && n >= 0) {
+      const float sn = Elem<kBF16>::to_f(sc[n]), sp = Elem<kBF16>::to_f(sc[t]);
+      if (re_hinge(a.margin, sn, sp) >= 0.f) {     // torch.clamp passes the gradient at 0
+        const float gn = re_sigmoid(sn), gp = re_sigmoid(sp);
+        if (re_live(a.obj_masks, b, n, len, Smax)) re_ds[n] = gn * (1.f - gn) * g;
+        if (re_live(a.obj_masks, b, static_cast<int>(t), len, Smax)) re_ds[t] = -gp * (1.f - gp) * g;
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int k = 0; k < Smax; ++k) s += re_ds[k];
+    part_b[b] = s;
+  }
+  const uint4* wv = reinterpret_cast<const uint4*>(a.weight);
+  const T16* rows = reinterpret_cast<const T16*>(a.rows);
+  T16* drows = reinterpret_cast<T16*>(a.d_rows);
+  const int nvec = H >> 3;
+  for (int v = threadIdx.x; v < nvec; v += RE_THREADS) {
+    float w[8], acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    h_unpack8<kBF16>(__ldg(wv + v), w);
+    for (int k = 0; k < len; ++k) {
+      const long long r = static_cast<long long>(start + k) * H;
+      const float d = re_ds[k];
+      float h[8], o[8];
+      h_unpack8<kBF16>(__ldg(reinterpret_cast<const uint4*>(rows + r) + v), h);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        acc[e] = fmaf(d, h[e], acc[e]);
+        o[e] = d * w[e];
+      }
+      reinterpret_cast<uint4*>(drows + r)[v] = h_pack8<kBF16>(o);
+    }
+    float4* pw = reinterpret_cast<float4*>(part_w + static_cast<long long>(b) * H + v * 8);
+    pw[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    pw[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+  }
+  const int gap_end = b + 1 < a.batch ? a.seg_start[b + 1] : a.R;
+  const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+  auto zero_rows = [&](int lo, int hi) {
+    for (long long i = static_cast<long long>(lo) * nvec + threadIdx.x; i < static_cast<long long>(hi) * nvec;
+         i += RE_THREADS)
+      reinterpret_cast<uint4*>(drows)[i] = zero;
+  };
+  zero_rows(start + len, gap_end);
+  if (b == 0) zero_rows(0, start);
+}
+
+// dweight[c] = sum_b part_w[b, c], dbias = sum_b part_b[b]: one thread per column, samples in order.
+__global__ void __launch_bounds__(RE_THREADS)
+region_score_wsum_kernel(const float* __restrict__ part_w, int batch, int H, float* __restrict__ dw,
+                         float* __restrict__ db) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int c = blockIdx.x * RE_THREADS + threadIdx.x;
+  if (c > H) return;
+  const float* src = c < H ? part_w + c : part_w + static_cast<long long>(batch) * H;
+  const int stride = c < H ? H : 1;
+  float s = 0.f;
+  for (int b = 0; b < batch; ++b) s += src[static_cast<long long>(b) * stride];
+  if (c < H) dw[c] = s; else if (db != nullptr) db[0] = s;
+}
+
 }  // namespace ub
 
 // ------------------------------------------------------------------------------ C ABI
@@ -554,5 +747,72 @@ extern "C" int ub200_adamw_step_scaled(const ub200_adam_segment* segs_dev, const
   ProfScope ps(stream);
   UB_CHECK_CUDA(launch_pdl(adamw_kernel, dim3(nblocks), dim3(256), 0, stream, 1, segs_dev, blk_start_dev,
                            nseg, h));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------ referring expressions
+extern "C" int64_t ub200_region_score_workspace_bytes(int32_t batch, int32_t hidden) {
+  return batch > 0 && hidden > 0 ? static_cast<int64_t>(batch) * (hidden + 1) * 4 : 0;
+}
+
+static int re_check(const ub200_region_score_args* a, const char* who) {
+  using namespace ub;
+  UB_CHECK_ARG(a && a->rows && a->weight && a->seg_start && a->seg_len && a->obj_masks && a->scores,
+               "%s: null pointer", who);
+  UB_CHECK_ARG(a->batch > 0 && a->R >= 0 && a->hidden > 0 && a->hidden % 8 == 0, "%s: need batch > 0, R >= 0 and "
+               "hidden a positive multiple of 8", who);
+  UB_CHECK_ARG(a->max_regions > 0 && a->max_regions <= RE_MAX_REGIONS, "%s: max_regions %d outside [1, %d]", who,
+               a->max_regions, RE_MAX_REGIONS);
+  UB_CHECK_ARG(a->mode == UB200_RE_SCORES || a->mode == UB200_RE_CLS || a->mode == UB200_RE_RANK,
+               "%s: unknown mode %d", who, a->mode);
+  UB_CHECK_ARG(a->dtype == UB200_F16 || a->dtype == UB200_BF16, "%s: dtype must be F16 or BF16", who);
+  UB_CHECK_ARG(((reinterpret_cast<uintptr_t>(a->rows) | reinterpret_cast<uintptr_t>(a->weight)) & 15) == 0,
+               "%s: rows and weight must be 16-byte aligned", who);
+  UB_CHECK_ARG(a->mode == UB200_RE_SCORES || a->targets, "%s: the losses need targets", who);
+  return 0;
+}
+
+extern "C" int ub200_region_score_fwd(const ub200_region_score_args* a, ub200_stream_t stream_) {
+  using namespace ub;
+  if (int rc = re_check(a, "region_score_fwd")) return rc;
+  UB_CHECK_ARG(a->mode == UB200_RE_SCORES || a->loss, "region_score_fwd: the losses need loss");
+  UB_CHECK_ARG(a->mode != UB200_RE_CLS || a->lse, "region_score_fwd: cls needs lse");
+  UB_CHECK_ARG(a->mode != UB200_RE_RANK || (a->neg_plan && a->neg_ix), "region_score_fwd: rank needs neg_plan "
+               "and neg_ix");
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const size_t smem = static_cast<size_t>(a->max_regions) * sizeof(float);
+  ProfScope ps(stream);
+  if (a->dtype == UB200_BF16)
+    UB_CHECK_CUDA(launch_pdl(region_score_fwd_kernel<true>, dim3(a->batch), dim3(RE_THREADS), smem, stream, 1, *a));
+  else
+    UB_CHECK_CUDA(launch_pdl(region_score_fwd_kernel<false>, dim3(a->batch), dim3(RE_THREADS), smem, stream, 1, *a));
+  return 0;
+}
+
+extern "C" int ub200_region_score_bwd(const ub200_region_score_args* a, ub200_stream_t stream_) {
+  using namespace ub;
+  if (int rc = re_check(a, "region_score_bwd")) return rc;
+  UB_CHECK_ARG(a->mode != UB200_RE_SCORES, "region_score_bwd: needs a loss mode");
+  UB_CHECK_ARG(a->dloss && a->d_rows && a->dweight && a->workspace, "region_score_bwd: null pointer");
+  UB_CHECK_ARG(a->mode != UB200_RE_CLS || a->lse, "region_score_bwd: cls needs lse");
+  UB_CHECK_ARG(a->mode != UB200_RE_RANK || a->neg_ix, "region_score_bwd: rank needs neg_ix");
+  UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->d_rows) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->workspace) & 15) == 0,
+               "region_score_bwd: d_rows and workspace must be 16-byte aligned");
+  UB_CHECK_ARG(a->workspace_bytes >= ub200_region_score_workspace_bytes(a->batch, a->hidden),
+               "region_score_bwd: workspace of %lld bytes, %lld needed", (long long)a->workspace_bytes,
+               (long long)ub200_region_score_workspace_bytes(a->batch, a->hidden));
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const size_t smem = static_cast<size_t>(a->max_regions) * sizeof(float);
+  {
+    ProfScope ps(stream);
+    if (a->dtype == UB200_BF16)
+      UB_CHECK_CUDA(launch_pdl(region_score_bwd_kernel<true>, dim3(a->batch), dim3(RE_THREADS), smem, stream, 1, *a));
+    else
+      UB_CHECK_CUDA(launch_pdl(region_score_bwd_kernel<false>, dim3(a->batch), dim3(RE_THREADS), smem, stream, 1, *a));
+  }
+  ProfScope ps(stream);
+  const int grid = (a->hidden + 1 + RE_THREADS - 1) / RE_THREADS;
+  UB_CHECK_CUDA(launch_pdl(region_score_wsum_kernel, dim3(grid), dim3(RE_THREADS), 0, stream, 1,
+                           static_cast<const float*>(a->workspace), a->batch, a->hidden, a->dweight, a->dbias));
   return 0;
 }

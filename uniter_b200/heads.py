@@ -13,9 +13,13 @@ Parameter names and module trees follow the reference so its checkpoints load
 * ``UniterForVisualQuestionAnswering`` (model/vqa.py:16-52) and ``UniterForImageTextRetrieval``
   (model/itm.py:14-59): pooler + small classifier, plain torch on top of the encoder — they are
   here so the parity tests can check head-level logits against the reference's goldens.
+* ``UniterForReferringExpressionComprehension`` (model/re.py): the region rows gathered from the
+  packed output, scored and turned into the per-sample loss by one fused kernel per direction.
 """
+import random
 from collections import defaultdict
 
+import numpy as np
 import torch
 from torch import nn
 from torch.nn import functional as F
@@ -480,3 +484,150 @@ class UniterForImageTextRetrievalHardNeg(UniterForImageTextRetrieval):
             register_lengths(masks, lens_sel, prefix=True)
         return {"sample_size": k + 1, "input_ids": ids, "position_ids": pos, "img_feat": feat,
                 "img_pos_feat": box, "attn_masks": masks, "gather_index": gather}
+
+
+# ============================================================================ referring expressions
+def re_neg_plan(targets, num_bbs, hard_ratio, np_random=None, py_random=None):
+    """The negative of each sample of the ranking loss, drawn like model/re.py:102-127 (sample_neg_ix):
+    per sample one np.random.uniform(0, 1, 1) draw decides hard (< hard_ratio) or easy; an easy sample
+    draws random.randint(0, num_bb - 1) until it differs from the target.  Returns a list with -1 for a
+    hard negative (the kernel picks the best-scoring other region on the device) and the drawn index for
+    an easy one.  By default the draws come from the same global generators as the reference's, so a
+    run seeded like train_re.py makes the same decisions; np_random / py_random replace them."""
+    nr = np_random if np_random is not None else np.random
+    pr = py_random if py_random is not None else random
+    plan = []
+    for t, nbb in zip(targets, num_bbs):
+        t, nbb = int(t), int(nbb)
+        if nbb < 2 or not 0 <= t < nbb:
+            raise ValueError("the ranking loss needs num_bb >= 2 and 0 <= target < num_bb, got target %d of %d"
+                             % (t, nbb))
+        if nr.uniform(0, 1, 1) < hard_ratio:
+            plan.append(-1)
+        else:
+            ix = pr.randint(0, nbb - 1)
+            while ix == t:
+                ix = pr.randint(0, nbb - 1)
+            plan.append(ix)
+    return plan
+
+
+class _RegionScoreHead(torch.autograd.Function):
+    """re_output (Linear(H, 1)) over the region rows, masked_fill(obj_masks, -1e4) and the per-sample
+    loss (model/re.py:69-96) in one kernel per direction (ub200_region_score_*).  Returns the loss [B]
+    fp32, or the masked scores [B, S] for mode RE_SCORES.  The weight and bias gradients are summed in
+    sample order and written into the gradient arena when the parameters live in one."""
+
+    @staticmethod
+    @_lib.forward_in_mode()
+    def forward(ctx, rows, weight, bias, seg, obj_masks, targets, neg_plan, mode, margin):
+        w = weight.reshape(-1)
+        if w.data_ptr() % 16:
+            w = w.clone()
+        scores, loss, lse, neg = ops.region_score_fwd(rows, w, bias, seg, obj_masks, targets, neg_plan,
+                                                      mode, margin)
+        if mode == _lib.RE_SCORES:
+            ctx.mark_non_differentiable(scores)
+            return scores
+        ctx.save_for_backward(rows, w, seg, obj_masks, targets, scores, lse, neg)
+        ctx.mode, ctx.margin, ctx.params = mode, margin, (weight, bias)
+        return loss
+
+    @staticmethod
+    @_lib.backward_in_mode
+    def backward(ctx, dloss):
+        rows, w, seg, obj_masks, targets, scores, lse, neg = ctx.saved_tensors
+        weight, bias = ctx.params
+        d_rows, dw, db = ops.region_score_bwd(rows, w, seg, obj_masks, targets, scores, lse, neg,
+                                              dloss.contiguous().float(), ctx.mode, ctx.margin)
+        dtype = rows.dtype
+        arena = getattr(weight, "_ub_arena", None)
+        params = [weight, bias]
+        if arena is not None and arena._still_valid() and all(id(p) in arena._views for p in params):
+            arena.mark_managed(params)
+            acc = arena.claim(params)
+            ops.cvt_from_f32(dw, dtype, out=arena.view(weight), accumulate=acc)
+            ops.cvt_from_f32(db, dtype, out=arena.view(bias), accumulate=acc)
+            return d_rows, None, None, None, None, None, None, None, None
+        return (d_rows, ops.cvt_from_f32(dw, dtype).view_as(weight), ops.cvt_from_f32(db, dtype).view_as(bias),
+                None, None, None, None, None, None)
+
+
+class UniterForReferringExpressionComprehension(UniterPreTrainedModel):
+    """model/re.py:18-100 on the packed path.  Same parameter names (`re_output.weight / bias`, or
+    `re_output.{0,2,3}.*` for mlp=2) and forward(batch, compute_loss) contract: the per-sample loss [B]
+    (fp32; cross-entropy for loss="cls", the ranking hinge for "rank") when training with
+    compute_loss, else the masked scores [B, max_num_bb].
+
+    The region rows are gathered straight from the packed encoder output (no padded [B, L, H] tensor,
+    no per-sample slicing); region k of sample b is padded position b * L + txt_lens[b] + k.  The batch
+    may carry, as batching.re_collate makes them, `re_index` (those flat positions, padded with B * L)
+    and `re_seg` (int32 [2, B]: start and length of each sample's rows); otherwise they are formed on
+    the host from `txt_lens` / `num_bbs`.  The ranking loss reads the plan of negatives from
+    `re_neg_plan` (int64 [B], see re_neg_plan) or, without one, draws it from the targets (one device
+    read, as model/re.py:112 does).  With all three keys the step reads nothing from the device and can
+    be captured by GraphedStep.  obj_masks may be uint8 (what data/re.py builds) or bool."""
+
+    def __init__(self, config, img_dim, loss="cls", margin=0.2, hard_ratio=0.3, mlp=1):
+        super().__init__(config)
+        self.uniter = UniterModel(config, img_dim)
+        H = config.hidden_size
+        if mlp == 1:
+            self.re_output = nn.Linear(H, 1)
+        elif mlp == 2:
+            self.re_output = nn.Sequential(nn.Linear(H, H), GELU(), nn.LayerNorm(H, eps=1e-12), nn.Linear(H, 1))
+        else:
+            raise ValueError("MLP restricted to be 1 or 2 layers.")
+        self.loss = loss
+        assert self.loss in ("cls", "rank")
+        if self.loss == "rank":
+            self.margin = margin
+            self.hard_ratio = hard_ratio
+        self.mlp = mlp
+        self.apply(self.init_weights)
+
+    def forward(self, batch, compute_loss=True):
+        from .batching import re_region_index
+        batch = defaultdict(lambda: None, batch)
+        packed, meta = self.uniter.encode_packed(
+            batch["input_ids"], batch["position_ids"], batch["img_feat"], batch["img_pos_feat"],
+            batch["attn_masks"], batch["gather_index"], output_all_encoded_layers=False)
+        dev = packed.device
+        num_bbs = batch["num_bbs"]
+        if num_bbs is not None and min(num_bbs) < 1:
+            raise ValueError("every sample needs at least one region, got num_bbs %s" % list(num_bbs))
+        index, seg = batch["re_index"], batch["re_seg"]
+        if index is None or seg is None:
+            if batch["txt_lens"] is None or num_bbs is None:
+                raise ValueError("the batch needs re_index and re_seg, or txt_lens and num_bbs")
+            index, seg = re_region_index(batch["txt_lens"], num_bbs, meta["L"])
+            index, seg = index.to(dev), seg.to(dev)
+        rows = gather_packed_rows(packed, meta["unpack_ext"][index])     # model/re.py:63-65
+        head = self.re_output
+        if self.mlp == 2:
+            rows = LibTransform.apply(rows, head[0].weight, head[0].bias, head[2].weight, head[2].bias)
+            head = head[3]
+        obj_masks = batch["obj_masks"]
+        if obj_masks.dtype not in (torch.uint8, torch.bool):
+            obj_masks = obj_masks != 0
+        obj_masks = obj_masks.contiguous()
+        if not compute_loss:
+            return _RegionScoreHead.apply(rows, head.weight, head.bias, seg, obj_masks, None, None,
+                                          _lib.RE_SCORES, 0.0)
+        targets = batch["targets"].reshape(-1)
+        if not targets.is_cuda and num_bbs is not None:
+            for t, nbb in zip(targets.tolist(), num_bbs):
+                if not 0 <= t < nbb:
+                    raise ValueError("target %d outside [0, %d)" % (t, nbb))
+        targets = targets.to(dev).contiguous()
+        if self.loss == "cls":
+            return _RegionScoreHead.apply(rows, head.weight, head.bias, seg, obj_masks, targets, None,
+                                          _lib.RE_CLS, 0.0)
+        plan = batch["re_neg_plan"]
+        if plan is None:
+            if num_bbs is None:
+                raise ValueError("the ranking loss needs re_neg_plan or num_bbs")
+            plan = torch.tensor(re_neg_plan(targets.tolist(), num_bbs, self.hard_ratio), dtype=torch.long)
+        plan = plan.to(dev).contiguous()
+        return _RegionScoreHead.apply(rows, head.weight, head.bias, seg, obj_masks, targets, plan,
+                                      _lib.RE_RANK, float(self.margin))

@@ -278,6 +278,68 @@ def dtanh_mul(dy, y):
     return out
 
 
+def _region_args(rows, weight, seg, obj_masks, mode, margin):
+    """Shared fields of ub200_region_score_args.  seg: int32 [2, B] (starts, lengths); obj_masks:
+    [B, S] uint8 or bool, non-zero = masked."""
+    assert rows.dim() == 2 and rows.is_contiguous() and weight.is_contiguous()
+    assert seg.dtype == torch.int32 and seg.is_contiguous() and seg.dim() == 2 and seg.size(0) == 2
+    assert obj_masks.dtype in (torch.uint8, torch.bool) and obj_masks.is_contiguous()
+    B, S = obj_masks.shape
+    assert seg.size(1) == B
+    return _lib.RegionScoreArgs(
+        rows=rows.data_ptr(), weight=weight.data_ptr(), seg_start=seg[0].data_ptr(), seg_len=seg[1].data_ptr(),
+        obj_masks=obj_masks.data_ptr(), R=rows.size(0), hidden=rows.size(1), batch=B, max_regions=S,
+        mode=int(mode), dtype=_lib.dtype_code(rows.dtype), margin=float(margin))
+
+
+@_follows_torch
+def region_score_fwd(rows, weight, bias, seg, obj_masks, targets=None, neg_plan=None, mode=_lib.RE_SCORES,
+                     margin=0.0):
+    """Referring-expression scores [B, S] (16-bit, masked positions = -1e4) and, for mode RE_CLS /
+    RE_RANK, the per-sample loss [B] fp32 with what the backward needs: lse [B] fp32 (cls) or the chosen
+    negative neg_ix [B] int32 (rank).  targets / neg_plan: int64 [B] (neg_plan -1 = hard negative)."""
+    lib = _lib.load()
+    a = _region_args(rows, weight, seg, obj_masks, mode, margin)
+    B, S = obj_masks.shape
+    dev = rows.device
+    scores = torch.empty(B, S, device=dev, dtype=rows.dtype)
+    loss = lse = neg = None
+    a.bias, a.scores = _lib.ptr(bias), scores.data_ptr()
+    if mode != _lib.RE_SCORES:
+        assert targets.dtype == torch.int64 and targets.is_contiguous() and targets.numel() == B
+        loss = torch.empty(B, device=dev, dtype=torch.float32)
+        a.targets, a.loss = targets.data_ptr(), loss.data_ptr()
+    if mode == _lib.RE_CLS:
+        lse = torch.empty(B, device=dev, dtype=torch.float32)
+        a.lse = lse.data_ptr()
+    elif mode == _lib.RE_RANK:
+        assert neg_plan.dtype == torch.int64 and neg_plan.is_contiguous() and neg_plan.numel() == B
+        neg = torch.empty(B, device=dev, dtype=torch.int32)
+        a.neg_plan, a.neg_ix = neg_plan.data_ptr(), neg.data_ptr()
+    _lib.check(lib.ub200_region_score_fwd(C.byref(a), _lib.current_stream()))
+    return scores, loss, lse, neg
+
+
+@_follows_torch
+def region_score_bwd(rows, weight, seg, obj_masks, targets, scores, lse, neg, dloss, mode, margin=0.0):
+    """Backward of region_score_fwd: d_rows [R, H] (16-bit, zero on padding rows), dweight [H] and
+    dbias [1] in fp32 (written, summed in sample order)."""
+    lib = _lib.load()
+    a = _region_args(rows, weight, seg, obj_masks, mode, margin)
+    B, H = obj_masks.size(0), rows.size(1)
+    assert dloss.dtype == torch.float32 and dloss.is_contiguous() and dloss.numel() == B
+    d_rows = torch.empty_like(rows)
+    dw = torch.empty(H, device=rows.device, dtype=torch.float32)
+    db = torch.empty(1, device=rows.device, dtype=torch.float32)
+    ws_bytes = lib.ub200_region_score_workspace_bytes(B, H)
+    ws = torch.empty(ws_bytes // 4, device=rows.device, dtype=torch.float32)
+    a.targets, a.scores, a.lse, a.neg_ix = targets.data_ptr(), scores.data_ptr(), _lib.ptr(lse), _lib.ptr(neg)
+    a.dloss, a.d_rows, a.dweight, a.dbias = dloss.data_ptr(), d_rows.data_ptr(), dw.data_ptr(), db.data_ptr()
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws_bytes
+    _lib.check(lib.ub200_region_score_bwd(C.byref(a), _lib.current_stream()))
+    return d_rows, dw, db
+
+
 @_follows_torch
 def gather_rows(src, index, rows=None):
     """dst[r] = src[index[r]] if index[r] >= 0 else 0 (int32 index; bit-exact row mover)."""
