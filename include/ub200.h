@@ -213,9 +213,20 @@ int64_t ub200_attn_bwd_workspace_bytes(int32_t total_tokens, int32_t hidden, int
  * the Philox stream used by the forward GEMM epilogue) and that Linear's bias gradient.
  * ub200_gather_rows is the bit-exact row mover behind pack / unpack and the gather_index
  * compaction of model/model.py:330-333:  dst[r] = index[r] >= 0 ? src[index[r]] : 0.
+ *
+ * Rows are up to 2048 columns wide (hidden % 8 == 0).  act = UB200_LN_ACT_RELU normalises relu(x)
+ * instead of x: y = LN(relu(pre)), the Linear(H, 2H) -> ReLU -> LayerNorm(2H) of the VCR head
+ * (model/vcr.py:27-32), with `pre` the Linear's 16-bit output.  Its backward takes pre as `x` and
+ * writes dpre = dx o (pre > 0) to dx_drop (required; dropout_p must be 0), with dbias = the column sums
+ * of dpre.  ReLU rows and rows wider than 1024 take the split form (stats_ws required) on plain rows.
  * ------------------------------------------------------------------------------------------ */
+#define UB200_LN_ACT_NONE 0
+#define UB200_LN_ACT_RELU 1
+
 int ub200_layernorm_fwd(const void* x, const void* gamma, const void* beta, void* y, int32_t rows,
                         int32_t hidden, int32_t dtype, ub200_stream_t stream);
+int ub200_layernorm_fwd_act(const void* x, const void* gamma, const void* beta, void* y, int32_t rows,
+                            int32_t hidden, int32_t dtype, int32_t act, ub200_stream_t stream);
 
 typedef struct {
   const void* dy;     /* [rows, hidden] */
@@ -238,6 +249,7 @@ typedef struct {
   float* stats_ws;          /* optional scratch, rows x 2 floats: selects the split form (a row kernel that
                                carries nothing between rows + a column-reduction kernel) for the plain
                                case (no row_kind, dropout on the Linear branch); NULL = one fused kernel */
+  int32_t act;              /* UB200_LN_ACT_NONE, or UB200_LN_ACT_RELU: x is pre of y = LN(relu(pre)) */
 } ub200_ln_bwd_args;
 int ub200_layernorm_bwd(const ub200_ln_bwd_args* args, ub200_stream_t stream);
 

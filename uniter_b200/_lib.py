@@ -56,8 +56,11 @@ class LnBwdArgs(C.Structure):
         ("rows", C.c_int32), ("hidden", C.c_int32), ("dtype", C.c_int32),
         ("dropout_p", C.c_float), ("rng_seed", C.c_uint64), ("rng_stream", C.c_uint64),
         ("row_kind", C.c_void_p), ("kind", C.c_int32), ("dropout_on_dy", C.c_int32),
-        ("rng_offset_dev", C.c_void_p), ("stats_ws", C.c_void_p),
+        ("rng_offset_dev", C.c_void_p), ("stats_ws", C.c_void_p), ("act", C.c_int32),
     ]
+
+
+LN_ACT_NONE, LN_ACT_RELU = 0, 1
 
 
 class EmbedPrepArgs(C.Structure):
@@ -163,6 +166,9 @@ def load():
     lib.ub200_layernorm_fwd.restype = C.c_int
     lib.ub200_layernorm_fwd.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_void_p]
+    lib.ub200_layernorm_fwd_act.restype = C.c_int
+    lib.ub200_layernorm_fwd_act.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.ub200_layernorm_bwd.restype = C.c_int
     lib.ub200_layernorm_bwd.argtypes = [C.POINTER(LnBwdArgs), C.c_void_p]
     lib.ub200_colsum.restype = C.c_int

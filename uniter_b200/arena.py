@@ -92,6 +92,10 @@ class GradArena(object):
             e._bind_arena(self, ep)
         self.step_mode = False
         self._fresh = set()
+        # the planned parameters themselves: their ids key the views, so none of them may be freed and
+        # its id reused by another tensor while this arena exists
+        self._planned = [p for p, _, _ in plan]
+        self._stale = False
         root._ub_arena = self
 
     # ------------------------------------------------------------------ lookup
@@ -117,7 +121,15 @@ class GradArena(object):
             a = GradArena(root)
         return a
 
+    def invalidate(self):
+        """Mark this arena as describing a parameter set that no longer exists (a parameter was replaced,
+        e.g. by the VCR head's init_type_embedding / init_word_embedding).  The next backward builds a
+        fresh arena; a GraphedStep built over this one refuses to run."""
+        self._stale = True
+
     def _still_valid(self):
+        if self._stale:
+            return False
         for e in self.encoders:
             p = e.encoder.layer[0].attention.self.query.weight
             if p.dtype != self.dtype or p.device != self.device:
@@ -125,7 +137,11 @@ class GradArena(object):
         return True
 
     def view(self, p):
-        return self._views[id(p)]
+        v = self._views.get(id(p))
+        if v is None or v.shape != p.shape:
+            raise RuntimeError("GradArena: a parameter of shape %s has no view in this gradient arena (was it "
+                               "replaced after the arena was built?)" % (tuple(p.shape),))
+        return v
 
     def segment(self, name):
         lo, hi = self.segments[name]

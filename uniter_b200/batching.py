@@ -13,6 +13,8 @@ GPU path run without a single device->host read:
   masked tokens, in the order of the reference's boolean-mask selection, model/pretrain.py:129-133).
 * ``re_collate`` / ``re_eval_collate`` — data/re.py:146-188, :251-295, plus ``re_index`` / ``re_seg``, the
   flat positions of the region rows and each sample's start and count in them (``re_region_index``).
+* ``vcr_collate`` / ``vcr_eval_collate`` — data/vcr.py:162-196, :262-300: every question contributes one
+  sequence per choice (4 answers; for eval also the 16 rationale sequences), flattened in order.
 * ``DevicePrefetcher`` — data/loader.py:86-141 (side-stream H2D of pinned batches, joined with
   ``wait_stream`` + ``record_stream``), additionally registering the per-sample lengths of the
   device attention mask with the model (``register_lengths``) so forward() never syncs.
@@ -177,6 +179,37 @@ def re_eval_collate(inputs):
      sent_ids) = map(list, zip(*inputs))
     batch = _re_fields(input_ids, img_feats, img_pos_feats, attn_masks, obj_masks)
     batch["tgt_box"], batch["obj_boxes"], batch["sent_ids"] = tgt_box, obj_boxes, sent_ids
+    return batch
+
+
+def _vcr_fields(input_ids, txt_type_ids, img_feats, img_pos_feats, attn_masks):
+    """The joint fields plus txt_type_ids padded with 0 (data/vcr.py:166-168)."""
+    batch = _joint_fields(input_ids, img_feats, img_pos_feats, attn_masks)
+    out = {"input_ids": batch.pop("input_ids"),
+           "txt_type_ids": pad_sequence(txt_type_ids, batch_first=True, padding_value=0)}
+    out.update(batch)
+    return out
+
+
+def vcr_collate(inputs):
+    """inputs: one tuple per question of (input_ids, txt_type_ids, img_feat, img_pos_feat, attn_masks,
+    target [1]) per choice — data/vcr.py:162-196 (VcrDataset).  targets: [n_choices_total, 1]."""
+    (input_ids, txt_type_ids, img_feats, img_pos_feats, attn_masks,
+     targets) = map(list, zip(*[c for q in inputs for c in q]))
+    batch = _vcr_fields(input_ids, txt_type_ids, img_feats, img_pos_feats, attn_masks)
+    batch["targets"] = torch.stack(targets, dim=0)
+    return batch
+
+
+def vcr_eval_collate(inputs):
+    """inputs: one (choices, qid, qa_target [1], qar_target [1]) per question, choices a tuple of
+    (input_ids, txt_type_ids, img_feat, img_pos_feat, attn_masks) — data/vcr.py:262-300 (VcrEvalDataset)."""
+    (input_ids, txt_type_ids, img_feats, img_pos_feats,
+     attn_masks) = map(list, zip(*[c for outs, _, _, _ in inputs for c in outs]))
+    batch = _vcr_fields(input_ids, txt_type_ids, img_feats, img_pos_feats, attn_masks)
+    batch["qa_targets"] = torch.stack([t for _, _, t, _ in inputs], dim=0)
+    batch["qar_targets"] = torch.stack([t for _, _, _, t in inputs], dim=0)
+    batch["qids"] = [qid for _, qid, _, _ in inputs]
     return batch
 
 

@@ -3,6 +3,8 @@
 //                 biased variance, eps inside the sqrt — model/layer.py:108,114,149,155)
 //   ln_bwd        dx (and dropout-masked dx), dgamma, dbeta, column-sum of the masked dx
 //                 (= bias gradient of the Linear that fed the residual sum), one pass
+//   ReLU rows     y = LayerNorm(relu(pre)) and its backward (dpre = dx o (pre > 0) in the masked-output
+//                 slot): the Linear(H, 2H) -> ReLU -> LayerNorm(2H) prefix of the VCR head (model/vcr.py)
 //   gather_rows   dst[r] = idx[r] >= 0 ? src[idx[r]] : 0     (pack / unpack between the padded
 //                 [B, L, H] view of the reference API and the packed [T, H] layout; bit-exact)
 //   colsum        out[n] += sum_m x[m, n]                       (bias gradient of the QKV projection)
@@ -17,6 +19,12 @@
 namespace ub {
 
 constexpr int LN_MAX_VEC = 4;  // per lane: 4 x 8 columns -> H <= 1024
+// Rows wider than 1024 columns (up to 2048) and ReLU-input rows run their own instantiations with
+// NV = 4, 6 or 8 vectors per lane (ln_wide_nv); the H <= 1024 plain-row kernels are left as they are.
+constexpr int LN_WIDE_MAX_VEC = 8;  // H <= 2048
+__host__ __device__ constexpr int ln_wide_nv(int H) {
+  return H <= 4 * 256 ? 4 : (H <= 6 * 256 ? 6 : 8);
+}
 constexpr float LN_EPS = 1e-12f;
 
 template <bool kBF16>
@@ -34,6 +42,14 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
   u.z = Elem<kBF16>::pack(f[4], f[5]); u.w = Elem<kBF16>::pack(f[6], f[7]);
   return u;
 }
+// relu of eight packed 16-bit values (fp16 or bf16: the sign is bit 15): every value with the sign bit
+// set becomes +0, the others are kept bit for bit.
+__device__ __forceinline__ uint32_t relu16x2(uint32_t u) {
+  return u & ~(((u >> 15) & 0x00010001u) * 0xFFFFu);
+}
+__device__ __forceinline__ uint4 relu16x8(uint4 u) {
+  return make_uint4(relu16x2(u.x), relu16x2(u.y), relu16x2(u.z), relu16x2(u.w));
+}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -41,8 +57,11 @@ __device__ __forceinline__ float warp_sum(float v) {
 }
 
 // ------------------------------------------------------------------------------ LayerNorm fwd
-template <bool kBF16>
-__global__ void __launch_bounds__(256)
+// kRelu: y = LayerNorm(relu(x)); relu of a 16-bit value is exact, so the statistics see exactly the
+// values torch's ReLU would hand to the LayerNorm.  (The ReLU instantiations state a minimum of one CTA
+// per SM: with no minimum, ptxas keeps them at 48-80 registers and spills.)
+template <bool kBF16, int NV = LN_MAX_VEC, bool kRelu = false>
+__global__ void __launch_bounds__(256, kRelu ? 1 : 0)
 ln_fwd_kernel(const void* __restrict__ x_, const void* __restrict__ gamma_,
               const void* __restrict__ beta_, void* __restrict__ y_, int rows, int H) {
   pdl_launch_dependents();
@@ -54,13 +73,13 @@ ln_fwd_kernel(const void* __restrict__ x_, const void* __restrict__ gamma_,
   const int nvec = H >> 3;
   const uint4* x = reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(x_) +
                                                   static_cast<size_t>(row) * H);
-  float v[LN_MAX_VEC][8];
+  float v[NV][8];
   float sum = 0.f;
 #pragma unroll
-  for (int i = 0; i < LN_MAX_VEC; ++i) {
+  for (int i = 0; i < NV; ++i) {
     const int vi = lane + i * 32;
     if (vi < nvec) {
-      unpack8<kBF16>(__ldg(x + vi), v[i]);
+      unpack8<kBF16>(kRelu ? relu16x8(__ldg(x + vi)) : __ldg(x + vi), v[i]);
 #pragma unroll
       for (int e = 0; e < 8; ++e) sum += v[i][e];
     }
@@ -68,7 +87,7 @@ ln_fwd_kernel(const void* __restrict__ x_, const void* __restrict__ gamma_,
   const float mean = warp_sum(sum) / H;
   float sq = 0.f;
 #pragma unroll
-  for (int i = 0; i < LN_MAX_VEC; ++i)
+  for (int i = 0; i < NV; ++i)
     if (lane + i * 32 < nvec) {
 #pragma unroll
       for (int e = 0; e < 8; ++e) { const float d = v[i][e] - mean; sq += d * d; }
@@ -78,7 +97,7 @@ ln_fwd_kernel(const void* __restrict__ x_, const void* __restrict__ gamma_,
   const uint4* bt = reinterpret_cast<const uint4*>(beta_);
   uint4* y = reinterpret_cast<uint4*>(reinterpret_cast<T16*>(y_) + static_cast<size_t>(row) * H);
 #pragma unroll
-  for (int i = 0; i < LN_MAX_VEC; ++i) {
+  for (int i = 0; i < NV; ++i) {
     const int vi = lane + i * 32;
     if (vi < nvec) {
       float gg[8], bb[8], o[8];
@@ -299,8 +318,11 @@ ln_bwd_kernel(const LnBwdParams p) {
 //                       per SM): dx, the dropout-masked copy, and (mean, rstd) of the row to `stats`;
 //   ln_bwd_cols_kernel  dgamma / dbeta / dbias as column reductions over a [64 columns x row slab]
 //                       block per CTA (the operands are L2-hot), 12x fewer atomics per address.
-template <bool kBF16, int NV>
-__global__ void __launch_bounds__(256, 2)
+// kRelu: x is the pre-activation `pre` of y = LN(relu(pre)); xhat comes from relu(pre) and dx_drop
+// receives dpre = dx o (pre > 0) (plain rows only: no dropout, no row kind).  Rows wider than 1024
+// (NV > 4) keep 16 x NV floats per thread and run one CTA per SM.
+template <bool kBF16, int NV, bool kRelu = false>
+__global__ void __launch_bounds__(256, NV > 4 ? 1 : 2)
 ln_bwd_rows_kernel(const LnBwdParams p, float2* __restrict__ stats) {
   pdl_launch_dependents();
   pdl_wait();
@@ -322,6 +344,7 @@ ln_bwd_rows_kernel(const LnBwdParams p, float2* __restrict__ stats) {
   if (p.drop_thr16) rng_add_dev_offset(p.rng_dev, rng.s0, rng.s1);
   rng.thr16 = p.drop_thr16; rng.inv_keep = p.drop_inv_keep;
   float xv[NV][8], dv[NV][8];
+  uint32_t live[kRelu ? NV : 1];   // kRelu: bit e of live[i] = (pre > 0) for column 8 * vi + e
   float sum = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
@@ -331,6 +354,14 @@ ln_bwd_rows_kernel(const LnBwdParams p, float2* __restrict__ stats) {
                                                           static_cast<size_t>(row) * H) + vi), xv[i]);
       unpack8<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.dy) +
                                                           static_cast<size_t>(row) * H) + vi), dv[i]);
+      if constexpr (kRelu) {
+        live[i] = 0u;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          if (xv[i][e] > 0.f) live[i] |= 1u << e;
+          else xv[i][e] = 0.f;
+        }
+      }
 #pragma unroll
       for (int e = 0; e < 8; ++e) sum += xv[i][e];
       if (p.dy_drop) {               // y = dropout(LN(x)) (deterministic mode only): mask dy
@@ -380,7 +411,11 @@ ln_bwd_rows_kernel(const LnBwdParams p, float2* __restrict__ stats) {
 #pragma unroll
       for (int e = 0; e < 8; ++e) o[e] = rstd * (dv[i][e] - s1 - xv[i][e] * s2);
       dxr[vi] = pack8<kBF16>(o);
-      if (ddr) {
+      if constexpr (kRelu) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) o[e] = ((live[i] >> e) & 1u) ? o[e] : 0.f;
+        ddr[vi] = pack8<kBF16>(o);
+      } else if (ddr) {
         const uint64_t el = static_cast<uint64_t>(row) * H + vi * 8;
         const uint4 rnd = rng.draw8(el >> 3);
 #pragma unroll
@@ -391,8 +426,8 @@ ln_bwd_rows_kernel(const LnBwdParams p, float2* __restrict__ stats) {
   }
 }
 
-// CTA = 8 column vectors (64 columns) x 32 row lanes over rows [r0, r1).
-template <bool kBF16>
+// CTA = 8 column vectors (64 columns) x 32 row lanes over rows [r0, r1).  kRelu: xhat from relu(x).
+template <bool kBF16, bool kRelu = false>
 __global__ void __launch_bounds__(256)
 ln_bwd_cols_kernel(const LnBwdParams p, const float2* __restrict__ stats, int rows_per_cta) {
   pdl_launch_dependents();
@@ -416,6 +451,10 @@ ln_bwd_cols_kernel(const LnBwdParams p, const float2* __restrict__ stats, int ro
                                                           static_cast<size_t>(r) * H + col0)), x);
       unpack8<kBF16>(__ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(p.dy) +
                                                           static_cast<size_t>(r) * H + col0)), dy);
+      if constexpr (kRelu) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) x[e] = x[e] > 0.f ? x[e] : 0.f;
+      }
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         ag[e] = fmaf(dy[e], (x[e] - st.x) * st.y, ag[e]);
@@ -453,7 +492,8 @@ ln_bwd_cols_kernel(const LnBwdParams p, const float2* __restrict__ stats, int ro
 // Deterministic form of ln_bwd_cols_kernel: CTA = 8 columns x 256 row lanes over ALL rows, so every
 // column has one owner and a fixed summation order (det_tree_sum8).  Also covers the row-kind and
 // dropout-on-dy cases of the embedding front-end (the fused kernel's job in the default mode).
-template <bool kBF16>
+// kRelu: xhat from relu(x), as ln_bwd_cols_kernel.
+template <bool kBF16, bool kRelu = false>
 __global__ void __launch_bounds__(256, 1)   // (256) alone: ptxas caps it at 64 registers and spills
 ln_bwd_cols_det_kernel(const LnBwdParams p, const float2* __restrict__ stats) {
   pdl_launch_dependents();
@@ -481,6 +521,10 @@ ln_bwd_cols_det_kernel(const LnBwdParams p, const float2* __restrict__ stats) {
       const uint4 rnd = rng.draw8(off >> 3);
 #pragma unroll
       for (int e = 0; e < 8; ++e) dy[e] = (rand16_of(rnd, e) < rng.thr16) ? 0.f : dy[e] * rng.inv_keep;
+    }
+    if constexpr (kRelu) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) x[e] = x[e] > 0.f ? x[e] : 0.f;
     }
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
@@ -627,15 +671,31 @@ add16_kernel(uint4* __restrict__ dst, const uint4* __restrict__ a, const uint4* 
 }
 
 // ------------------------------------------------------------------------------ launchers
+template <bool kBF16, bool kRelu>
+static cudaError_t launch_ln_fwd_nv(const void* x, const void* gamma, const void* beta, void* y, int rows,
+                                    int H, int grid, cudaStream_t stream) {
+  switch (ln_wide_nv(H)) {
+    case 4: return launch_pdl(ln_fwd_kernel<kBF16, 4, kRelu>, dim3(grid), dim3(256), 0, stream, 1, x, gamma, beta, y, rows, H);
+    case 6: return launch_pdl(ln_fwd_kernel<kBF16, 6, kRelu>, dim3(grid), dim3(256), 0, stream, 1, x, gamma, beta, y, rows, H);
+    default: return launch_pdl(ln_fwd_kernel<kBF16, 8, kRelu>, dim3(grid), dim3(256), 0, stream, 1, x, gamma, beta, y, rows, H);
+  }
+}
+
 int launch_ln_fwd(int dtype, const void* x, const void* gamma, const void* beta, void* y, int rows,
-                  int H, cudaStream_t stream) {
-  if (H % 8 != 0 || H > LN_MAX_VEC * 256 || rows <= 0)
+                  int H, bool relu, cudaStream_t stream) {
+  if (H % 8 != 0 || H > LN_WIDE_MAX_VEC * 256 || rows <= 0)
     return set_error(UB200_EUNSUPPORTED, "ln_fwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
-                     LN_MAX_VEC * 256, H);
+                     LN_WIDE_MAX_VEC * 256, H);
   const int grid = (rows + 7) / 8;
   ProfScope ps(stream);
-  if (dtype == UB200_BF16) UB_CHECK_CUDA(launch_pdl(ln_fwd_kernel<true>, dim3(grid), dim3(256), 0, stream, 1, x, gamma, beta, y, rows, H));
-  else UB_CHECK_CUDA(launch_pdl(ln_fwd_kernel<false>, dim3(grid), dim3(256), 0, stream, 1, x, gamma, beta, y, rows, H));
+  const bool bf = dtype == UB200_BF16;
+  if (relu) {
+    if (bf) UB_CHECK_CUDA((launch_ln_fwd_nv<true, true>(x, gamma, beta, y, rows, H, grid, stream)));
+    else UB_CHECK_CUDA((launch_ln_fwd_nv<false, true>(x, gamma, beta, y, rows, H, grid, stream)));
+  } else {
+    if (bf) UB_CHECK_CUDA((launch_ln_fwd_nv<true, false>(x, gamma, beta, y, rows, H, grid, stream)));
+    else UB_CHECK_CUDA((launch_ln_fwd_nv<false, false>(x, gamma, beta, y, rows, H, grid, stream)));
+  }
   UB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -652,46 +712,53 @@ static cudaError_t launch_ln_bwd_nv(const LnBwdParams& p, int grid, cudaStream_t
 }
 
 template <bool kBF16>
-static cudaError_t launch_ln_bwd_rows_nv(const LnBwdParams& p, float2* stats, int grid, cudaStream_t stream) {
+static cudaError_t launch_ln_bwd_rows_nv(const LnBwdParams& p, bool relu, float2* stats, int grid,
+                                         cudaStream_t stream) {
+  if (relu) {
+    switch (ln_wide_nv(p.H)) {
+      case 4: return launch_pdl(ln_bwd_rows_kernel<kBF16, 4, true>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
+      case 6: return launch_pdl(ln_bwd_rows_kernel<kBF16, 6, true>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
+      default: return launch_pdl(ln_bwd_rows_kernel<kBF16, 8, true>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
+    }
+  }
   const int nv = (p.H + 255) / 256;
   switch (nv) {
     case 1: return launch_pdl(ln_bwd_rows_kernel<kBF16, 1>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
     case 2: return launch_pdl(ln_bwd_rows_kernel<kBF16, 2>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
     case 3: return launch_pdl(ln_bwd_rows_kernel<kBF16, 3>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
-    default: return launch_pdl(ln_bwd_rows_kernel<kBF16, 4>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
+    case 4: return launch_pdl(ln_bwd_rows_kernel<kBF16, 4>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
+    case 5:
+    case 6: return launch_pdl(ln_bwd_rows_kernel<kBF16, 6>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
+    default: return launch_pdl(ln_bwd_rows_kernel<kBF16, 8>, dim3(grid), dim3(256), 0, stream, 1, p, stats);
   }
 }
 
+template <bool kBF16, bool kRelu>
+static cudaError_t launch_ln_bwd_cols(const LnBwdParams& p, const float2* stats, cudaStream_t stream) {
+  if (deterministic())
+    return launch_pdl(ln_bwd_cols_det_kernel<kBF16, kRelu>, dim3(p.H / 8), dim3(256), 0, stream, 1, p, stats);
+  const int gx = (p.H + 63) / 64;
+  int gy = (2 * num_sms() + gx - 1) / gx;
+  if (gy > (p.rows + 31) / 32) gy = (p.rows + 31) / 32;
+  if (gy < 1) gy = 1;
+  const int rpc = (p.rows + gy - 1) / gy;
+  return launch_pdl(ln_bwd_cols_kernel<kBF16, kRelu>, dim3(gx, gy), dim3(256), 0, stream, 1, p, stats, rpc);
+}
+
 // split form (see ln_bwd_rows_kernel): needs `stats` = rows x 2 floats of caller-owned scratch
-int launch_ln_bwd_split(int dtype, const LnBwdParams& p, float* stats_ws, cudaStream_t stream) {
+int launch_ln_bwd_split(int dtype, const LnBwdParams& p, bool relu, float* stats_ws, cudaStream_t stream) {
   float2* stats = reinterpret_cast<float2*>(stats_ws);
   const bool bf = dtype == UB200_BF16;
   {
     ProfScope ps(stream);
     const int grid = (p.rows + 7) / 8;
-    if (bf) UB_CHECK_CUDA(launch_ln_bwd_rows_nv<true>(p, stats, grid, stream));
-    else UB_CHECK_CUDA(launch_ln_bwd_rows_nv<false>(p, stats, grid, stream));
+    if (bf) UB_CHECK_CUDA(launch_ln_bwd_rows_nv<true>(p, relu, stats, grid, stream));
+    else UB_CHECK_CUDA(launch_ln_bwd_rows_nv<false>(p, relu, stats, grid, stream));
   }
-  if (deterministic()) {
-    ProfScope ps(stream);
-    if (bf) UB_CHECK_CUDA(launch_pdl(ln_bwd_cols_det_kernel<true>, dim3(p.H / 8), dim3(256), 0, stream, 1, p,
-                                     static_cast<const float2*>(stats)));
-    else UB_CHECK_CUDA(launch_pdl(ln_bwd_cols_det_kernel<false>, dim3(p.H / 8), dim3(256), 0, stream, 1, p,
-                                  static_cast<const float2*>(stats)));
-    return 0;
-  }
-  {
-    const int gx = (p.H + 63) / 64;
-    int gy = (2 * num_sms() + gx - 1) / gx;
-    if (gy > (p.rows + 31) / 32) gy = (p.rows + 31) / 32;
-    if (gy < 1) gy = 1;
-    const int rpc = (p.rows + gy - 1) / gy;
-    ProfScope ps(stream);
-    if (bf) UB_CHECK_CUDA(launch_pdl(ln_bwd_cols_kernel<true>, dim3(gx, gy), dim3(256), 0, stream, 1, p,
-                                     static_cast<const float2*>(stats), rpc));
-    else UB_CHECK_CUDA(launch_pdl(ln_bwd_cols_kernel<false>, dim3(gx, gy), dim3(256), 0, stream, 1, p,
-                                  static_cast<const float2*>(stats), rpc));
-  }
+  ProfScope ps(stream);
+  const float2* st = stats;
+  if (bf) UB_CHECK_CUDA(relu ? (launch_ln_bwd_cols<true, true>(p, st, stream)) : (launch_ln_bwd_cols<true, false>(p, st, stream)));
+  else UB_CHECK_CUDA(relu ? (launch_ln_bwd_cols<false, true>(p, st, stream)) : (launch_ln_bwd_cols<false, false>(p, st, stream)));
   return 0;
 }
 
@@ -791,7 +858,16 @@ extern "C" int ub200_layernorm_fwd(const void* x, const void* gamma, const void*
                                    int32_t rows, int32_t hidden, int32_t dtype,
                                    ub200_stream_t stream) {
   UB_CHECK_ARG(x && gamma && beta && y, "layernorm_fwd: null pointer");
-  return ub::launch_ln_fwd(dtype, x, gamma, beta, y, rows, hidden,
+  return ub::launch_ln_fwd(dtype, x, gamma, beta, y, rows, hidden, false,
+                           reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int ub200_layernorm_fwd_act(const void* x, const void* gamma, const void* beta, void* y,
+                                       int32_t rows, int32_t hidden, int32_t dtype, int32_t act,
+                                       ub200_stream_t stream) {
+  UB_CHECK_ARG(x && gamma && beta && y, "layernorm_fwd_act: null pointer");
+  UB_CHECK_ARG(act == UB200_LN_ACT_NONE || act == UB200_LN_ACT_RELU, "layernorm_fwd_act: unknown act %d", act);
+  return ub::launch_ln_fwd(dtype, x, gamma, beta, y, rows, hidden, act == UB200_LN_ACT_RELU,
                            reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -821,20 +897,40 @@ extern "C" int ub200_layernorm_bwd(const ub200_ln_bwd_args* a, ub200_stream_t st
   p.stream_lo = static_cast<uint32_t>(a->rng_stream);
   p.stream_hi = static_cast<uint32_t>(a->rng_stream >> 32);
   p.rng_dev = reinterpret_cast<const unsigned long long*>(a->rng_offset_dev);
+  UB_CHECK_ARG(a->act == UB200_LN_ACT_NONE || a->act == UB200_LN_ACT_RELU, "layernorm_bwd: unknown act %d", a->act);
+  const bool relu = a->act == UB200_LN_ACT_RELU;
+  if (relu || p.H > ub::LN_MAX_VEC * 256) {
+    // ReLU rows and rows wider than 1024: always the split form (row kernel + column kernel, fixed-order
+    // in the deterministic mode), on plain rows.  With ReLU, dx_drop receives dpre = dx o (pre > 0).
+    UB_CHECK_ARG(a->stats_ws != nullptr, "layernorm_bwd: ReLU or hidden > %d needs stats_ws (rows x 2 floats)",
+                 ub::LN_MAX_VEC * 256);
+    UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
+    UB_CHECK_ARG(a->row_kind == nullptr && !(a->dropout_on_dy & 1),
+                 "layernorm_bwd: ReLU or hidden > %d takes no row_kind and no dropout on dy", ub::LN_MAX_VEC * 256);
+    if (relu) {
+      UB_CHECK_ARG(a->dx_drop != nullptr, "layernorm_bwd: ReLU needs dx_drop (it receives dpre)");
+      UB_CHECK_ARG(a->dropout_p == 0.f, "layernorm_bwd: ReLU and dropout share dx_drop; dropout_p must be 0");
+      p.dx_drop = a->dx_drop;
+    }
+    if (p.H % 8 != 0 || p.H > ub::LN_WIDE_MAX_VEC * 256 || p.rows <= 0)
+      return ub::set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
+                           ub::LN_WIDE_MAX_VEC * 256, p.H);
+    return ub::launch_ln_bwd_split(a->dtype, p, relu, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
+  }
   if (ub::deterministic()) {   // one form for every case: row kernel + fixed-order column kernel
     UB_CHECK_ARG(a->stats_ws != nullptr, "layernorm_bwd: deterministic mode needs stats_ws (rows x 2 floats)");
     UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
     if (p.H % 8 != 0 || p.H > ub::LN_MAX_VEC * 256 || p.rows <= 0)
       return ub::set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
                            ub::LN_MAX_VEC * 256, p.H);
-    return ub::launch_ln_bwd_split(a->dtype, p, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
+    return ub::launch_ln_bwd_split(a->dtype, p, false, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
   }
   if (a->stats_ws != nullptr && a->row_kind == nullptr && !p.dy_drop) {
     UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
     if (p.H % 8 != 0 || p.H > ub::LN_MAX_VEC * 256 || p.rows <= 0)
       return ub::set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
                            ub::LN_MAX_VEC * 256, p.H);
-    return ub::launch_ln_bwd_split(a->dtype, p, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
+    return ub::launch_ln_bwd_split(a->dtype, p, false, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
   }
   return ub::launch_ln_bwd(a->dtype, p, reinterpret_cast<cudaStream_t>(stream));
 }

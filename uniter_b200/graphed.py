@@ -303,4 +303,7 @@ class GraphedStep(object):
         return bk
 
     def __call__(self, batch, lens, accumulate=False, tag=None, step_optimizer=True):
+        if self.arena._stale:
+            raise RuntimeError("GraphedStep: parameters of the module were replaced after this step was built "
+                               "(e.g. by init_type_embedding / init_word_embedding); build a new GraphedStep")
         return self.replay(self.stage(batch, lens, accumulate, tag, step_optimizer))

@@ -15,6 +15,8 @@ Parameter names and module trees follow the reference so its checkpoints load
   here so the parity tests can check head-level logits against the reference's goldens.
 * ``UniterForReferringExpressionComprehension`` (model/re.py): the region rows gathered from the
   packed output, scored and turned into the per-sample loss by one fused kernel per direction.
+* ``UniterForVisualCommonsenseReasoning`` (model/vcr.py): the [CLS] rows gathered from the packed output,
+  the library pooler, LibTransform(act="relu") at twice the hidden size and LibLinear with N = 2.
 """
 import random
 from collections import defaultdict
@@ -180,20 +182,34 @@ class UniterForMLM(UniterPreTrainedModel):
 
 
 class LibTransform(torch.autograd.Function):
-    """z = LayerNorm(gelu(h W^T + b)) — BertPredictionHeadTransform (model/layer.py:188-203) and the
-    `net.0 / net.1 / net.2` prefix of RegionFeatureRegression / RegionClassification
-    (model/pretrain.py:19-47) — on libub200: GEMM with the bias + GELU epilogue, LayerNorm kernels,
-    dGELU kernel, dgrad / wgrad GEMMs.  Gradients of parameters that live in a gradient arena are
-    written there directly."""
+    """z = LayerNorm(act(h W^T + b)) on libub200, with act = "gelu" (default) or "relu".
+
+    gelu: BertPredictionHeadTransform (model/layer.py:188-203) and the `net.0 / net.1 / net.2` prefix of
+    RegionFeatureRegression / RegionClassification (model/pretrain.py:19-47): GEMM with the bias + GELU
+    epilogue, LayerNorm kernels, dGELU kernel, dgrad / wgrad GEMMs.
+    relu: the `vcr_output.0 / .1 / .2` prefix of the VCR head (model/vcr.py:27-32), Linear(H, 2H) ->
+    ReLU -> LayerNorm(2H): GEMM with the plain bias epilogue, then the LayerNorm kernels with the ReLU
+    applied as they load `pre`; their backward also writes dpre = dx o (pre > 0) and its column sums
+    (the Linear's bias gradient).
+
+    Gradients of parameters that live in a gradient arena are written there directly."""
 
     @staticmethod
     @_lib.forward_in_mode()
-    def forward(ctx, h, dense_w, dense_b, ln_g, ln_b):
+    def forward(ctx, h, dense_w, dense_b, ln_g, ln_b, act="gelu"):
+        if act not in ("gelu", "relu"):
+            raise ValueError("LibTransform: act must be 'gelu' or 'relu', got %r" % (act,))
         h = h.contiguous()
-        t, pre = ops.gemm(h, dense_w, bias=dense_b, gelu=True)
-        z = ops.layernorm_fwd(t, ln_g, ln_b)
+        if act == "relu":
+            pre = ops.gemm(h, dense_w, bias=dense_b)
+            t = pre
+            z = ops.layernorm_fwd(pre, ln_g, ln_b, relu=True)
+        else:
+            t, pre = ops.gemm(h, dense_w, bias=dense_b, gelu=True)
+            z = ops.layernorm_fwd(t, ln_g, ln_b)
         ctx.save_for_backward(h, pre, t)
         ctx.params = (dense_w, dense_b, ln_g, ln_b)
+        ctx.act = act
         return z
 
     @staticmethod
@@ -202,20 +218,26 @@ class LibTransform(torch.autograd.Function):
         h, pre, t = ctx.saved_tensors
         dense_w, dense_b, ln_g, ln_b = ctx.params
         dtype = h.dtype
-        dt, _, dg, db, _ = ops.layernorm_bwd(dz.contiguous(), t, ln_g, want_dbias=False)
-        dpre = ops.dgelu_mul(dt, pre)
+        if ctx.act == "relu":
+            _, dpre, dg, db, dbias = ops.layernorm_bwd(dz.contiguous(), pre, ln_g, relu=True)
+        else:
+            dt, _, dg, db, _ = ops.layernorm_bwd(dz.contiguous(), t, ln_g, want_dbias=False)
+            dpre = ops.dgelu_mul(dt, pre)
+            dbias = None
         dh = ops.gemm(dpre, dense_w, b_major=1) if ctx.needs_input_grad[0] else None
         arena = getattr(dense_w, "_ub_arena", None)
         if arena is not None and arena._still_valid() and all(id(q) in arena._views for q in ctx.params):
             arena.mark_managed(ctx.params)
             acc = arena.claim(list(ctx.params))
             ops.gemm(dpre, h, a_major=1, b_major=1, out=arena.view(dense_w), accumulate=acc)
-            ops.cvt_from_f32(ops.colsum(dpre), dtype, out=arena.view(dense_b), accumulate=acc)
+            ops.cvt_from_f32(ops.colsum(dpre) if dbias is None else dbias, dtype, out=arena.view(dense_b),
+                             accumulate=acc)
             ops.cvt_from_f32(dg, dtype, out=arena.view(ln_g), accumulate=acc)
             ops.cvt_from_f32(db, dtype, out=arena.view(ln_b), accumulate=acc)
-            return dh, None, None, None, None
-        return (dh, ops.gemm(dpre, h, a_major=1, b_major=1), ops.cvt_from_f32(ops.colsum(dpre), dtype),
-                ops.cvt_from_f32(dg, dtype), ops.cvt_from_f32(db, dtype))
+            return dh, None, None, None, None, None
+        return (dh, ops.gemm(dpre, h, a_major=1, b_major=1),
+                ops.cvt_from_f32(ops.colsum(dpre) if dbias is None else dbias, dtype),
+                ops.cvt_from_f32(dg, dtype), ops.cvt_from_f32(db, dtype), None)
 
 
 class RegionFeatureRegression(nn.Module):
@@ -631,3 +653,87 @@ class UniterForReferringExpressionComprehension(UniterPreTrainedModel):
         plan = plan.to(dev).contiguous()
         return _RegionScoreHead.apply(rows, head.weight, head.bias, seg, obj_masks, targets, plan,
                                       _lib.RE_RANK, float(self.margin))
+
+
+# ============================================================================ visual commonsense reasoning
+class UniterForVisualCommonsenseReasoning(UniterPreTrainedModel):
+    """model/vcr.py on the packed path.  Same parameter names (`vcr_output.{0,2,3}.*`), the same
+    forward(batch, compute_loss) contract (the mean cross-entropy over the batch, a scalar, with
+    compute_loss; else scores[:, 1:], shape [B, 1]) and the same init_type_embedding /
+    init_word_embedding semantics.
+
+    The [CLS] rows are gathered from the packed encoder output (as VQA and ITM do), the pooler is the
+    library's, and vcr_output runs as LibTransform(act="relu") — Linear(H, 2H) -> ReLU -> LayerNorm(2H)
+    with the ReLU fused into the LayerNorm kernels — then LibLinear(2H, 2).  txt_type_ids (values 0-3
+    after init_type_embedding) reach the embedding front-end.  With the host-known lengths registered
+    (batching.vcr_collate provides txt_lens / num_bbs) a step reads nothing from the device, so
+    GraphedStep captures it."""
+
+    def __init__(self, config, img_dim):
+        super().__init__(config, img_dim)
+        self.uniter = UniterModel(config, img_dim)
+        H = config.hidden_size
+        self.vcr_output = nn.Sequential(
+            nn.Linear(H, H * 2),
+            nn.ReLU(),
+            nn.LayerNorm(H * 2, eps=1e-12),
+            nn.Linear(H * 2, 2))
+        self.apply(self.init_weights)
+
+    def _replace_table(self, name, new_emb):
+        """Install new_emb (built and initialised on the CPU in fp32, as the reference does) as
+        uniter.embeddings.<name> on the old table's device and dtype, and retire every gradient arena
+        planned over the old parameter set."""
+        from .arena import GradArena
+        te = self.uniter.embeddings
+        old = getattr(te, name).weight
+        new_emb = new_emb.to(device=old.device, dtype=old.dtype)
+        new_emb.weight.requires_grad_(old.requires_grad)
+        stale = {id(a): a for a in (getattr(old, "_ub_arena", None), GradArena.of(self),
+                                    self.uniter._arena[0] if self.uniter._arena is not None else None)
+                 if a is not None}
+        for a in stale.values():
+            a.invalidate()
+        self.uniter._arena = None
+        setattr(te, name, new_emb)
+
+    def init_type_embedding(self):
+        """model/vcr.py:34-44: a 4-row token-type table, init_weights-initialised; rows 0 and 1 copied
+        from the old table, rows 2 and 3 copies of old row 0.  Consumes the global torch RNG like the
+        reference (the new table is built on the CPU in fp32 whatever the model's device)."""
+        old = self.uniter.embeddings.token_type_embeddings.weight.data.float().cpu()
+        new_emb = nn.Embedding(4, self.uniter.config.hidden_size)
+        new_emb.apply(self.init_weights)
+        for i in [0, 1]:
+            new_emb.weight.data[i, :].copy_(old[i, :])
+        new_emb.weight.data[2, :].copy_(old[0, :])
+        new_emb.weight.data[3, :].copy_(old[0, :])
+        self._replace_table("token_type_embeddings", new_emb)
+
+    def init_word_embedding(self, num_special_tokens):
+        """model/vcr.py:46-53: an nn.Embedding(V + num_special_tokens, H) with no padding_idx,
+        init_weights-initialised, its first V rows copied from the old table (train_vcr.py adds 81)."""
+        old = self.uniter.embeddings.word_embeddings.weight.data.float().cpu()
+        orig_word_num = old.size(0)
+        new_emb = nn.Embedding(orig_word_num + num_special_tokens, self.uniter.config.hidden_size)
+        new_emb.apply(self.init_weights)
+        new_emb.weight.data[:orig_word_num, :].copy_(old)
+        self._replace_table("word_embeddings", new_emb)
+
+    def forward(self, batch, compute_loss=True):
+        batch = defaultdict(lambda: None, batch)
+        packed, meta = self.uniter.encode_packed(
+            batch["input_ids"], batch["position_ids"], batch["img_feat"], batch["img_pos_feat"],
+            batch["attn_masks"], batch["gather_index"], output_all_encoded_layers=False,
+            txt_type_ids=batch["txt_type_ids"])
+        B, L = meta["n_batch"], meta["L"]
+        cls_rows = meta["unpack_ext"][::L][:B].contiguous()       # packed row of position (b, 0)
+        pooled_output = self.uniter.pooler(gather_packed_rows(packed, cls_rows))
+        head = self.vcr_output
+        hidden = LibTransform.apply(pooled_output, head[0].weight, head[0].bias, head[2].weight, head[2].bias,
+                                    "relu")
+        rank_scores = LibLinear.apply(hidden, head[3].weight, head[3].bias, False, False)
+        if compute_loss:
+            targets = batch["targets"]
+            return F.cross_entropy(rank_scores.float(), targets.squeeze(-1), reduction="mean")
+        return rank_scores[:, 1:]

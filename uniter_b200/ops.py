@@ -165,10 +165,16 @@ def _attn_bwd(qkv, ctx, lse, dctx, cu_seqlens, max_seqlen, num_heads, dropout_p,
 
 
 @_follows_torch
-def layernorm_fwd(x, gamma, beta):
+def layernorm_fwd(x, gamma, beta, relu=False):
+    """y = LayerNorm(x) (or LayerNorm(relu(x)) with relu) over rows of up to 2048 columns."""
     lib = _lib.load()
     rows, H = x.shape
     y = torch.empty_like(x)
+    if relu:
+        _lib.check(lib.ub200_layernorm_fwd_act(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(),
+                                               rows, H, _lib.dtype_code(x.dtype), _lib.LN_ACT_RELU,
+                                               _lib.current_stream()))
+        return y
     _lib.check(lib.ub200_layernorm_fwd(x.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(),
                                        rows, H, _lib.dtype_code(x.dtype), _lib.current_stream()))
     return y
@@ -177,14 +183,17 @@ def layernorm_fwd(x, gamma, beta):
 @_follows_torch
 def layernorm_bwd(dy, x, gamma, dropout_p=0.0, rng_seed=0, rng_stream=0, want_dbias=True,
                   row_kind=None, kind=0, dropout_on_dy=False, dx=None, dgamma=None, dbeta=None, dbias=None,
-                  zero_inactive=False, rng_offset_dev=None, split=False):
+                  zero_inactive=False, rng_offset_dev=None, split=False, relu=False):
     """Returns dx, dx_drop (or None), dgamma, dbeta, dbias (fp32).  split=True: row kernel + column
-    kernel (plain case only; in the deterministic mode every case is split)."""
+    kernel (plain case only; in the deterministic mode every case is split).
+    relu=True: x is `pre` of y = LayerNorm(relu(pre)); the second result is then dpre = dx o (pre > 0)
+    and dbias its column sums (no dropout, no row kind).  Rows wider than 1024 and ReLU rows always
+    take the split form."""
     lib = _lib.load()
     rows, H = x.shape
     if dx is None:
         dx = torch.empty_like(x) if row_kind is None else torch.zeros_like(x)
-    dx_drop = torch.empty_like(x) if (dropout_p > 0 and not dropout_on_dy) else None
+    dx_drop = torch.empty_like(x) if (relu or (dropout_p > 0 and not dropout_on_dy)) else None
     if dgamma is None:
         dgamma = torch.zeros(H, device=x.device, dtype=torch.float32)
     if dbeta is None:
@@ -197,8 +206,8 @@ def layernorm_bwd(dy, x, gamma, dropout_p=0.0, rng_seed=0, rng_stream=0, want_db
                        dropout_p=float(dropout_p), rng_seed=int(rng_seed), rng_stream=int(rng_stream),
                        row_kind=_lib.ptr(row_kind), kind=int(kind),
                        dropout_on_dy=(1 if dropout_on_dy else 0) | (2 if zero_inactive else 0),
-                       rng_offset_dev=rng_offset_dev)
-    if split or _lib.deterministic():   # the deterministic mode always takes the split form
+                       rng_offset_dev=rng_offset_dev, act=_lib.LN_ACT_RELU if relu else _lib.LN_ACT_NONE)
+    if split or relu or H > 1024 or _lib.deterministic():   # the deterministic mode always takes the split form
         ws = torch.empty(rows, 2, device=x.device, dtype=torch.float32)
         a.stats_ws = ws.data_ptr()
     _lib.check(lib.ub200_layernorm_bwd(C.byref(a), _lib.current_stream()))
