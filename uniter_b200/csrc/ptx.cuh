@@ -261,8 +261,14 @@ __device__ __forceinline__ float rcp_approx(float x) {
 }
 
 // Standard-normal CDF Phi(x) through erf(|x|/sqrt2) = 1 - poly(t) * exp(-x^2/2),
-// t = 1/(1 + p|x|/sqrt2)  (Abramowitz & Stegun 7.1.26, |abs err| <= 1.5e-7 — far below the
-// 16-bit output rounding).  `ex` returns exp(-x^2/2), shared with the pdf in the derivative.
+// t = 1/(1 + p|x|/sqrt2)  (Abramowitz & Stegun 7.1.26).  The formula's 1.5e-7 is an ABSOLUTE error
+// of erf; evaluated in fp32 with the MUFU forms below, Phi is within 4e-7 of the exact value (absolute,
+// tests/gemm_check.py DELTA_PHI, checked over every 16-bit x).  That is far below the 16-bit rounding
+// of gelu(x) = x Phi(x) wherever Phi is not small, but for x < -4 it is a large RELATIVE error of Phi
+// (about 3e-4 at -4, 4e-2 at -5; Phi is 0 below about -6): the GELU tail is accurate to |x| * 4e-7
+// absolute, still closer than the reference model's composed 16-bit GELU, whose 1 + erf is quantised
+// to the 16-bit spacing below 1 (it gives gelu(-4) = 0).  `ex` returns exp(-x^2/2), shared with the pdf
+// in the derivative.
 // The reciprocal and the exponential are the bare MUFU approximations (rcp.approx.ftz on an
 // argument >= 1, ex2.approx.ftz on x^2 * -log2(e)/2), without the range-handling FSETP / FMUL /
 // branch sequences __fdividef / __expf add: the GELU epilogues run once per output element and

@@ -57,7 +57,18 @@ def gemm(a, b, *, a_major=0, b_major=0, bias=None, residual=None, aux=None, out=
             out = torch.zeros(M, N, device=a.device, dtype=torch.float32)
         else:
             out = torch.empty(M, N, device=a.device, dtype=torch.float32 if out_fp32 else a.dtype)
-    out2 = torch.empty(M, N, device=a.device, dtype=a.dtype) if gelu else None
+    # the kernel reads and writes [M, N] at the row pitches it is given: check every side tensor here,
+    # before the launch, rather than let it touch memory outside them
+    for name, t, dt in (("out", out, None), ("residual", residual, a.dtype), ("aux", aux, a.dtype)):
+        if t is not None:
+            assert tuple(t.shape) == (M, N) and t.stride(1) == 1 and t.device == a.device, \
+                "%s must be [%d, %d] with unit column stride, got %s / %s" % (name, M, N, tuple(t.shape), t.stride())
+            assert dt is None or t.dtype == dt, "%s must be %s, got %s" % (name, dt, t.dtype)
+    assert out.dtype in (a.dtype, torch.float32), "out must be %s or float32, got %s" % (a.dtype, out.dtype)
+    assert bias is None or (bias.numel() == N and bias.dtype == a.dtype and bias.is_contiguous()), \
+        "bias must hold %d contiguous %s elements" % (N, a.dtype)
+    # out2 has out's row pitch (include/ub200.h): the kernel stores it at row * ldo + col
+    out2 = torch.empty(M, out.stride(0), device=a.device, dtype=a.dtype)[:, :N] if gelu else None
     epi = 0
     if bias is not None:
         epi |= EPI_BIAS
