@@ -105,12 +105,7 @@ int ub200_profile_collect(float* ms_per_tag, int* launches_per_tag, int ntags);
  *   UB200_EPI_COLSUM    colsum[n] += sum_m v  (fp32 atomics; bias gradients)
  *   UB200_EPI_ATOMIC    out[m,n] += v with fp32 atomics (requires OUT_F32 and a pre-zeroed out);
  *                       the only epilogue allowed with k_splits > 1 (split-K partial sums)
- *   UB200_EPI_LN        fused residual + LayerNorm (model/layer.py:111-115, :152-156): with
- *                       BIAS | RESIDUAL [| DROPOUT], K-major operands and N = 768 or 1024, `out` receives
- *                       s = dropout(acc + bias) + residual (saved for the backward) and
- *                       ln_out = LayerNorm(s) * ln_gamma + ln_beta (eps 1e-12, statistics of the 16-bit s
- *                       in fp32); the row is split over a 4-CTA cluster that exchanges (mean, M2)
- *                       through distributed shared memory
+ * Any other bit of `epilogue` is UB200_EINVAL.
  * ------------------------------------------------------------------------------------------ */
 enum {
   UB200_EPI_BIAS = 1,
@@ -123,7 +118,6 @@ enum {
   UB200_EPI_COLSUM = 128,
   UB200_EPI_ATOMIC = 256,
   UB200_EPI_TANH = 512,
-  UB200_EPI_LN = 1024,
 };
 
 typedef struct {
@@ -158,10 +152,6 @@ typedef struct {
   const uint64_t* rng_offset_dev; /* optional DEVICE counter: the dropout stream used is
                               rng_stream + (*rng_offset_dev << 20).  Lets a CUDA graph replay the same
                               launch with fresh masks (the host bumps the counter, not the arguments) */
-  const void* ln_gamma;    /* UB200_EPI_LN: [N] 16-bit */
-  const void* ln_beta;     /* UB200_EPI_LN: [N] 16-bit */
-  void* ln_out;            /* UB200_EPI_LN: [M, N] 16-bit, pitch ldln */
-  int64_t ldln;
 } ub200_gemm_args;
 
 int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream);

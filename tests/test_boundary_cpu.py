@@ -45,7 +45,7 @@ def test_library_exports_every_declared_symbol(lib):
     assert len(names) >= 20, names
     missing = [n for n in names if not hasattr(lib, n)]
     assert not missing, "declared in include/ub200.h but not exported: %s" % missing
-    assert lib.ub200_version() >= 100
+    assert lib.ub200_version() >= 200
 
 
 def test_library_has_no_libcuda_link_dependency():
@@ -66,6 +66,17 @@ def test_errors_are_reported_not_thrown(lib):
     assert b"NULL" in lib.ub200_last_error_string()
 
 
+def test_gemm_rejects_unknown_epilogue_bits(lib):
+    """An epilogue bit outside UB200_EPI_* is UB200_EINVAL, not a plain GEMM, and is reported before the
+    operands are touched on a device (they are not device pointers here)."""
+    from uniter_b200 import _lib
+    for bit in (1024, 2048):
+        args = _lib.GemmArgs(a=16, b=16, out=16, lda=64, ldb=64, ldo=64, M=128, N=64, K=64, dtype=_lib.BF16,
+                             epilogue=_lib.EPI_BIAS | bit, bias=16)
+        assert lib.ub200_gemm(C.byref(args), None) == -1, bit
+        assert b"epilogue" in lib.ub200_last_error_string()
+
+
 def test_ctypes_mirrors_match_the_header_layout():
     """Compile a tiny C program against include/ub200.h and compare sizeof() with ctypes."""
     from uniter_b200 import _lib
@@ -75,10 +86,11 @@ def test_ctypes_mirrors_match_the_header_layout():
     #include <stddef.h>
     #include "ub200.h"
     int main(void) {
-      printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\n", sizeof(ub200_gemm_args), sizeof(ub200_attn_args),
+      printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\n", sizeof(ub200_gemm_args), sizeof(ub200_attn_args),
              sizeof(ub200_ln_bwd_args), sizeof(ub200_layer_weights), sizeof(ub200_layer_grads),
              sizeof(ub200_encoder_desc), sizeof(ub200_adam_segment), sizeof(ub200_embed_colsum_args),
              offsetof(ub200_gemm_args, k_splits), offsetof(ub200_gemm_args, n_valid),
+             offsetof(ub200_gemm_args, rng_offset_dev),
              offsetof(ub200_adam_segment, step_size), offsetof(ub200_embed_colsum_args, T),
              sizeof(ub200_peer_allreduce_args), offsetof(ub200_peer_allreduce_args, stage_bytes));
       return 0;
@@ -92,10 +104,12 @@ def test_ctypes_mirrors_match_the_header_layout():
     mine = [C.sizeof(_lib.GemmArgs), C.sizeof(_lib.AttnArgs), C.sizeof(_lib.LnBwdArgs),
             C.sizeof(_LayerWeights), C.sizeof(_LayerGrads), C.sizeof(_EncoderDesc),
             C.sizeof(_lib.AdamSegment), C.sizeof(_lib.EmbedColsumArgs),
-            _lib.GemmArgs.k_splits.offset, _lib.GemmArgs.n_valid.offset,
+            _lib.GemmArgs.k_splits.offset, _lib.GemmArgs.n_valid.offset, _lib.GemmArgs.rng_offset_dev.offset,
             _lib.AdamSegment.step_size.offset, _lib.EmbedColsumArgs.T.offset,
             C.sizeof(_lib.PeerAllreduceArgs), _lib.PeerAllreduceArgs.stage_bytes.offset]
     assert sizes == mine, (sizes, mine)
+    # the layout of ub200_version() 200: ub200_gemm_args ends with rng_offset_dev
+    assert (sizes[0], sizes[10]) == (192, 184), sizes
 
 
 def _tiny_cfg():

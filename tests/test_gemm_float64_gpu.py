@@ -401,35 +401,6 @@ def test_random_every_mask_ragged(dtype, majors):
     assert not fails, fails
 
 
-@pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("M", [1, 129, 3451])
-@pytest.mark.parametrize("N", [768, 1024])
-def test_random_fused_layernorm(dtype, M, N):
-    """EPI_LN: s against the float64 chain, ln_out against float64 LayerNorm of the kernel's own s."""
-    from uniter_b200 import ops
-    K = 768
-    g = _gen(M + N)
-    a = torch.randn(M, K, generator=g, device=DEV).to(dtype)
-    w = (torch.randn(N, K, generator=g, device=DEV) * 0.05).to(dtype)
-    bias = (torch.randn(N, generator=g, device=DEV) * 0.1).to(dtype)
-    res = torch.randn(M, N, generator=g, device=DEV)
-    res[::7] += 40.0
-    res = res.to(dtype)
-    gamma = (1 + 0.1 * torch.randn(N, generator=g, device=DEV)).to(dtype)
-    beta = (0.1 * torch.randn(N, generator=g, device=DEV)).to(dtype)
-    counter = torch.tensor([2], device=DEV, dtype=torch.int64)
-    s, y = ops.gemm(a, w, bias=bias, residual=res, dropout_p=0.1, rng_seed=SEED, rng_stream=STREAM,
-                    rng_offset_dev=counter.data_ptr(), ln=(gamma, beta))
-    _sync()
-    keep, inv = rc.keep_mask(SEED, STREAM, 0.1, M, N, device=DEV, counter=2)
-    fails, stats = gc.check_gemm(dict(out=s), gc.gemm_reference(a, w), K, B | D | R, dtype, bias=bias, residual=res,
-                                 keep=keep, inv_keep=inv)
-    f, st = rc.check_rows("ln_out", y, rc.ln_fwd_reference(s, gamma, beta), rc.ln_fwd_baseline(s, gamma, beta), dtype)
-    print("RATIO fused-LN M=%d N=%d %s s=%.3f ln_worst_row=%.3f" % (M, N, str(dtype).split(".")[-1], stats["out"],
-                                                                    st.get("worst_row_ratio", 0)))
-    assert not fails + f, fails + f
-
-
 # ------------------------------------------------------------------------------------ (c) exhaustive
 def _all_finite(dtype):
     """Every finite 16-bit value, as a [256, 256] matrix (non-finite patterns replaced by 0)."""

@@ -16,7 +16,6 @@ EPI_BIAS, EPI_DROPOUT, EPI_RESIDUAL, EPI_GELU = 1, 2, 4, 8
 EPI_DGELU, EPI_ACCUM, EPI_OUT_F32, EPI_COLSUM = 16, 32, 64, 128
 EPI_ATOMIC = 256
 EPI_TANH = 512
-EPI_LN = 1024
 
 
 class GemmArgs(C.Structure):
@@ -34,7 +33,6 @@ class GemmArgs(C.Structure):
         ("tile_n", C.c_int32), ("max_ctas", C.c_int32), ("cluster", C.c_int32),
         ("k_splits", C.c_int32), ("n_valid", C.c_int32),
         ("rng_offset_dev", C.c_void_p),
-        ("ln_gamma", C.c_void_p), ("ln_beta", C.c_void_p), ("ln_out", C.c_void_p), ("ldln", C.c_int64),
     ]
 
 

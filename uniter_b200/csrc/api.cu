@@ -183,7 +183,7 @@ int ub200_profile_collect(float* ms_out, int* count_out, int ntags) {
 }
 
 
-int ub200_version(void) { return 100; /* 0.1.0 */ }
+int ub200_version(void) { return 200; /* 0.2.0 */ }
 
 const char* ub200_last_error_string(void) { return ub::g_err; }
 

@@ -1,8 +1,6 @@
 // Encoder-stack orchestration: enqueues the per-layer kernel sequence of NL BertLayers
 // (forward and backward) from C++ so that one C-ABI call covers the whole stack.
 // Reference: UniterEncoder.forward model/model.py:282-292, BertLayer model/layer.py:159-170.
-#include <stdlib.h>
-
 #include "common.h"
 
 namespace ub {
@@ -128,11 +126,6 @@ extern "C" int ub200_encoder_fwd(const ub200_encoder_desc* d, const ub200_layer_
   const ActLayout L(T, H, I, d->num_heads);
   uint8_t* act = reinterpret_cast<uint8_t*>(act_);
 
-  // residual + LayerNorm fused into the producing GEMM's epilogue where the row fits a 4-CTA cluster
-  // (H = 768 / 1024: both UNITER configs); UB200_FUSE_LN=0 selects the two-kernel path (A/B runs)
-  static const bool fuse_env = [] { const char* e = getenv("UB200_FUSE_LN"); return e && e[0] == '1'; }();
-  const bool fuse_ln = fuse_env && (H == 768 || H == 1024);
-
   const void* x = x_in;
   for (int l = 0; l < d->num_layers; ++l) {
     const ub200_layer_weights& w = layers[l];
@@ -167,14 +160,11 @@ extern "C" int ub200_encoder_fwd(const ub200_encoder_desc* d, const ub200_layer_
     g.epilogue = UB200_EPI_BIAS | UB200_EPI_RESIDUAL | (d->hidden_dropout_p > 0 ? UB200_EPI_DROPOUT : 0);
     g.bias = w.bo; g.residual = x; g.ldr = H; g.out = A + L.s1; g.ldo = H;
     g.dropout_p = d->hidden_dropout_p; g.rng_stream = rng_stream_of(d, l, SITE_ATTN_OUT);
-    if (fuse_ln) {   // LayerNorm in the GEMM epilogue (4-CTA cluster over the row)
-      g.epilogue |= UB200_EPI_LN; g.ln_gamma = w.ln1_g; g.ln_beta = w.ln1_b; g.ln_out = A + L.a; g.ldln = H;
-    }
     {
       ProfTag _t(3);
       UB_TRY(ub200_gemm(&g, stream));
     }
-    if (!fuse_ln) {
+    {
       ProfTag _t(4);
       UB_TRY(ub200_layernorm_fwd(A + L.s1, w.ln1_g, w.ln1_b, A + L.a, T, H, d->dtype, stream));
     }
@@ -195,14 +185,11 @@ extern "C" int ub200_encoder_fwd(const ub200_encoder_desc* d, const ub200_layer_
     g.epilogue = UB200_EPI_BIAS | UB200_EPI_RESIDUAL | (d->hidden_dropout_p > 0 ? UB200_EPI_DROPOUT : 0);
     g.bias = w.b2; g.residual = A + L.a; g.ldr = H; g.out = A + L.s2; g.ldo = H;
     g.dropout_p = d->hidden_dropout_p; g.rng_stream = rng_stream_of(d, l, SITE_FFN_OUT);
-    if (fuse_ln) {
-      g.epilogue |= UB200_EPI_LN; g.ln_gamma = w.ln2_g; g.ln_beta = w.ln2_b; g.ln_out = layer_out[l]; g.ldln = H;
-    }
     {
       ProfTag _t(6);
       UB_TRY(ub200_gemm(&g, stream));
     }
-    if (!fuse_ln) {
+    {
       ProfTag _t(7);
       UB_TRY(ub200_layernorm_fwd(A + L.s2, w.ln2_g, w.ln2_b, layer_out[l], T, H, d->dtype, stream));
     }
@@ -236,9 +223,8 @@ extern "C" int ub200_encoder_bwd(const ub200_encoder_desc* d, const ub200_layer_
   cudaStream_t cs = reinterpret_cast<cudaStream_t>(stream);
   const bool drop = d->hidden_dropout_p > 0.f;
   const int acc = accumulate_wgrad ? UB200_EPI_ACCUM : 0;
-  // UB200_LN_BWD_SPLIT=1: row kernel + column kernel instead of the fused LayerNorm backward (A/B runs)
-  static const bool ln_split = [] { const char* e = getenv("UB200_LN_BWD_SPLIT"); return e && e[0] == '1'; }();
-  float* ln_ws = (ln_split || deterministic()) ? reinterpret_cast<float*>(sc + S.ln_stats) : nullptr;
+  // the deterministic mode's LayerNorm backward (row kernel + fixed-order column kernel) needs stats_ws
+  float* ln_ws = deterministic() ? reinterpret_cast<float*>(sc + S.ln_stats) : nullptr;
 
   const void* dcur = d_layer_out[NL - 1];
   int pp = 0;  // ping-pong for the running gradient

@@ -1,7 +1,5 @@
 // C entry point of the wgmma GEMM core: argument checks, tile / cluster selection, TMA
 // descriptors.  Device code lives in gemm_impl.cuh (instantiated in gemm_bf16.cu / gemm_f16.cu).
-#include <stdlib.h>
-
 #include "common.h"
 
 #include "gemm_params.h"
@@ -13,8 +11,11 @@ int gemm_dispatch_f16(int bn, int cluster, int a_major, int b_major, const GemmP
                       const CUtensorMap& tmA, const CUtensorMap& tmB, int grid, cudaStream_t stream);
 int gemm_group_dispatch_bf16(const void* tm, const GroupedParams& g, int grid, cudaStream_t stream);
 int gemm_group_dispatch_f16(const void* tm, const GroupedParams& g, int grid, cudaStream_t stream);
-int launch_gemm_ln(int dtype, const GemmParams& p, const void* gamma, const void* beta, void* y,
-                   long long ldy, const CUtensorMap& tmA, const CUtensorMap& tmB, cudaStream_t stream);
+
+// Every UB200_EPI_* bit the epilogue implements; any other bit is an argument error.
+constexpr int EPI_KNOWN = UB200_EPI_BIAS | UB200_EPI_DROPOUT | UB200_EPI_RESIDUAL | UB200_EPI_GELU |
+                          UB200_EPI_DGELU | UB200_EPI_ACCUM | UB200_EPI_OUT_F32 | UB200_EPI_COLSUM |
+                          UB200_EPI_ATOMIC | UB200_EPI_TANH;
 
 // Pick (N tile, CTAs per tile) minimising the modelled time in microseconds:
 //   waves x (k-blocks x per_kb(bn, cluster) + per_tile(bn, cluster)).
@@ -68,6 +69,7 @@ extern "C" int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream_) {
   UB_CHECK_ARG(a.dtype == UB200_F16 || a.dtype == UB200_BF16, "gemm: bad dtype %d", a.dtype);
   UB_CHECK_ARG(a.N % 8 == 0 && a.ldo % 8 == 0, "gemm: N and ldo must be multiples of 8");
   const int epi = a.epilogue;
+  UB_CHECK_ARG((epi & ~EPI_KNOWN) == 0, "gemm: unknown epilogue bits 0x%x", epi & ~EPI_KNOWN);
   UB_CHECK_ARG(!(epi & UB200_EPI_BIAS) || a.bias, "gemm: EPI_BIAS without bias");
   UB_CHECK_ARG(!(epi & UB200_EPI_RESIDUAL) || (a.residual && a.ldr % 8 == 0),
                "gemm: EPI_RESIDUAL needs residual with ldr %% 8 == 0");
@@ -101,47 +103,6 @@ extern "C" int ub200_gemm(const ub200_gemm_args* args, ub200_stream_t stream_) {
     const int rc = ub200_gemm(&b, stream_);
     if (rc || !(epi & UB200_EPI_COLSUM)) return rc;
     return launch_colsum_det(a.dtype, a.out, a.colsum, a.M, a.N, a.ldo, stream);
-  }
-
-  if (epi & UB200_EPI_LN) {
-    // fused residual + LayerNorm epilogue: its own kernel (4-CTA cluster over N), see gemm_ln.cu
-    const int allowed = UB200_EPI_LN | UB200_EPI_BIAS | UB200_EPI_RESIDUAL | UB200_EPI_DROPOUT;
-    UB_CHECK_ARG((epi & ~allowed) == 0 && (epi & UB200_EPI_BIAS) && (epi & UB200_EPI_RESIDUAL),
-                 "gemm: EPI_LN combines with BIAS | RESIDUAL [| DROPOUT] only");
-    UB_CHECK_ARG(a.a_major == 0 && a.b_major == 0, "gemm: EPI_LN needs K-major operands");
-    UB_CHECK_ARG(a.ln_gamma && a.ln_beta && a.ln_out && a.ldln % 8 == 0, "gemm: EPI_LN needs ln_gamma / ln_beta / ln_out");
-    if (a.N != 768 && a.N != 1024)
-      return set_error(UB200_EUNSUPPORTED, "gemm: EPI_LN needs N = 768 or 1024 (got %d)", a.N);
-    const int bnl = a.N / 4;
-    CUtensorMap tmA, tmB;
-    int rc = make_tma_2d(&tmA, a.a, a.dtype, a.M, a.K, a.lda, BM, BK);
-    if (rc) return rc;
-    rc = make_tma_2d(&tmB, a.b, a.dtype, a.N, a.K, a.ldb, bnl, BK);
-    if (rc) return rc;
-    GemmParams p{};
-    p.M = a.M; p.N = a.N; p.K = a.K;
-    p.epilogue = epi;
-    p.bias = a.bias; p.residual = a.residual; p.out = a.out;
-    p.ldr = a.ldr; p.ldo = a.ldo;
-    if ((epi & UB200_EPI_DROPOUT) && a.dropout_p > 0.f) {
-      const DropoutThreshold d = dropout_threshold(a.dropout_p);
-      p.drop_thr16 = d.thr16;
-      p.drop_inv_keep = d.inv_keep;
-    } else {
-      p.epilogue &= ~UB200_EPI_DROPOUT;
-      p.drop_thr16 = 0;
-      p.drop_inv_keep = 1.f;
-    }
-    p.seed_lo = static_cast<uint32_t>(a.rng_seed);
-    p.seed_hi = static_cast<uint32_t>(a.rng_seed >> 32);
-    p.stream_lo = static_cast<uint32_t>(a.rng_stream);
-    p.stream_hi = static_cast<uint32_t>(a.rng_stream >> 32);
-    p.rng_dev = reinterpret_cast<const unsigned long long*>(a.rng_offset_dev);
-    p.tiles_m = (a.M + BM - 1) / BM;
-    p.tiles_n = 4;
-    p.ksplit = 1;
-    p.kb_per_split = (a.K + BK - 1) / BK;
-    return launch_gemm_ln(a.dtype, p, a.ln_gamma, a.ln_beta, a.ln_out, a.ldln, tmA, tmB, stream);
   }
 
   const int sms = num_sms();
@@ -239,10 +200,6 @@ extern "C" int ub200_gemm_grouped(const ub200_gemm_args* args, int32_t count, ub
   // an unmeasured heuristic, not part of pick_config's fit: wider tiles cost less per column).
   const int sms = num_sms();
   int bn = args[0].tile_n;
-  if (bn == 0) {
-    static const int env_bn = [] { const char* e = getenv("UB200_GROUP_BN"); return e ? atoi(e) : 0; }();
-    bn = env_bn;
-  }
   if (bn == 0) {
     double best = 1e30;
     const int cand[3] = {128, 192, 256};

@@ -37,26 +37,11 @@ namespace ub {
 
 constexpr int A_TILE_BYTES = BM * BK * 2;
 
-// Register-epilogue layout (gemm_ln.cu): producer + 2 consumer warpgroups, the consumers run the
-// epilogue from their accumulators through a per-warp 16 x 32 transpose buffer.
-constexpr int GEMM_THREADS = 384;
-constexpr int EPI_WARPS = 8;            // consumer warps, 16 accumulator rows each
-constexpr int EPI_PITCH = 33;           // fp32 words per row of a warp's 16 x 32 transpose buffer
-
-template <int BN>
-struct GemmCfg {
-  static constexpr int B_TILE_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
-  static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
-  static constexpr int BAR_BYTES = 256;
-  static constexpr int EPI_STAGE_BYTES = EPI_WARPS * 16 * EPI_PITCH * 4;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + EPI_STAGE_BYTES + 1024;  // + align slack
-};
-
-// Epilogue-warpgroup layout (gemm_kernel, gemm_group_kernel): the TMA ring, then the ring of fp32
+// Shared-memory layout (gemm_kernel, gemm_group_kernel): the TMA ring, then the ring of fp32
 // hand-off chunks (128 rows x 64 columns each), then the mbarriers.  The chunks take the shared
 // memory of one TMA stage: 5 stages at BN = 128, 4 at 192, 3 at 256.
 constexpr int GEMM_WS_THREADS = 512;    // producer + 2 consumer + epilogue warpgroups
+constexpr int CONSUMER_WARPS = 8;       // 16 accumulator rows each; all 8 fill every chunk
 constexpr int CHUNK_COLS = 64;
 constexpr int CHUNK_BYTES = BM * CHUNK_COLS * 4;
 constexpr int EPI_CHUNKS = 2;           // one whole 128-wide tile
@@ -64,7 +49,7 @@ constexpr int MAX_DYN_SMEM = 227 * 1024;
 
 template <int BN>
 struct WsCfg {
-  static constexpr int STAGE_BYTES = GemmCfg<BN>::STAGE_BYTES;
+  static constexpr int STAGE_BYTES = A_TILE_BYTES + BN * BK * 2;
   static constexpr int RING_BYTES = EPI_CHUNKS * CHUNK_BYTES;
   static constexpr int BAR_BYTES = 256;
   static constexpr int FIT = (MAX_DYN_SMEM - RING_BYTES - BAR_BYTES - 1024) / STAGE_BYTES;
@@ -72,6 +57,11 @@ struct WsCfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + RING_BYTES + BAR_BYTES + 1024;  // + align slack
   static_assert((2 * STAGES + 2 * EPI_CHUNKS) * 8 <= BAR_BYTES, "mbarriers overflow their region");
 };
+static_assert(WsCfg<64>::STAGES == 6 && WsCfg<128>::STAGES == 5 && WsCfg<192>::STAGES == 4 &&
+              WsCfg<256>::STAGES == 3, "TMA ring depth per tile width");
+static_assert(WsCfg<64>::SMEM_BYTES == 214272 && WsCfg<128>::SMEM_BYTES == 230656 &&
+              WsCfg<192>::SMEM_BYTES == 230656 && WsCfg<256>::SMEM_BYTES == 214272,
+              "dynamic shared memory per tile width");
 
 template <bool kBF16>
 __device__ __forceinline__ void load8(const void* base, long long idx, float (&f)[8]) {
@@ -118,19 +108,6 @@ struct EpiMask {
     return EPI >= 0 ? (EPI & bit) != 0 : (rt & bit) != 0;
   }
 };
-
-// Register-epilogue transpose (gemm_ln.cu): the fragment scatters a row over 4 lanes in 2-column
-// pieces, so each 16 x 32 block of a warp goes through smem (pitch 33 words), after which 4 lanes
-// own one row.
-template <int BN>
-__device__ __forceinline__ void stage_block(const float (&acc)[BN / 2], int c, int lane, float* stage) {
-#pragma unroll
-  for (int t = 0; t < 16; ++t) {
-    const int r = (lane >> 2) + 8 * ((t >> 1) & 1);
-    const int cc = 8 * (t >> 2) + 2 * (lane & 3) + (t & 1);
-    stage[r * EPI_PITCH + cc] = acc[16 * c + t];
-  }
-}
 
 // Word of element (r, c) in a 128 x 64 fp32 hand-off chunk.  Rows are 64 words; the 16-byte column
 // groups are XOR-swizzled by (r & 3) << 1 | (r & 1), so that the consumers' fragment writes (a
@@ -323,12 +300,6 @@ __device__ __forceinline__ DropoutRng make_rng(const GemmParams& p) {
   return rng;
 }
 
-__device__ __forceinline__ void setmaxnreg_producer() {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-}
-__device__ __forceinline__ void setmaxnreg_consumer() {
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
-}
 // 512-thread kernels start at 128 registers a thread: 24 + 2 x 192 + 104 = 4 x 128
 __device__ __forceinline__ void setmaxnreg_ws_producer() {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
@@ -342,13 +313,12 @@ __device__ __forceinline__ void setmaxnreg_ws_epilogue() {
 
 // ------------------------------------------------------------------------------ pipeline halves
 // Producer lane: k-blocks [kb0, kb1) of the 128 x BN tile at (m0, n0) into the ring.  With
-// kCluster = 2 this CTA (cluster rank `rank`) loads half of the B tile and multicasts it.  The ring
-// has kStages stages.
-template <int BN, bool A_MN, bool B_MN, int kCluster, int kStages = GemmCfg<BN>::STAGES>
+// kCluster = 2 this CTA (cluster rank `rank`) loads half of the B tile and multicasts it.
+template <int BN, bool A_MN, bool B_MN, int kCluster>
 __device__ __forceinline__ void produce_tile(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                              const CUtensorMap* tmA, const CUtensorMap* tmB, int m0, int n0,
                                              int kb0, int kb1, int& stage, uint32_t& phase, uint32_t rank) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = WsCfg<BN>;
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(&empty_bar[stage], phase ^ 1);
     uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
@@ -381,20 +351,18 @@ __device__ __forceinline__ void produce_tile(uint8_t* smem, uint64_t* full_bar, 
         }
       }
     }
-    if (++stage == kStages) { stage = 0; phase ^= 1; }
+    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
   }
 }
 
 // Consumer warpgroup `wg` (rows [64 wg, 64 wg + 64) of the tile): acc = A B^T over nkb k-blocks.
 // K-major operands advance 16 elements = 32 B inside the swizzle row per k16 step; MN-major ones
 // advance 16 K-rows = 2048 B, their 64-wide M/N groups are one 8 KB box apart.
-// kHalves256: issue a 256-wide tile as two m64n128 wgmmas (the 512-thread kernels, see below).
-template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster, int kStages = GemmCfg<BN>::STAGES,
-          bool kHalves256 = false>
+template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster>
 __device__ __forceinline__ void consume_tile(float (&acc)[BN / 2], uint8_t* smem, uint64_t* full_bar,
                                              uint64_t* empty_bar, int nkb, int wg, int& stage,
                                              uint32_t& phase, uint32_t peer) {
-  using Cfg = GemmCfg<BN>;
+  using Cfg = WsCfg<BN>;
   constexpr uint32_t A_KSTEP = A_MN ? 2048 : 32, A_LBO = A_MN ? 8192 : 16;
   constexpr uint32_t B_KSTEP = B_MN ? 2048 : 32, B_LBO = B_MN ? 8192 : 16;
   const bool releaser = (threadIdx.x & 127) == 0;
@@ -408,7 +376,7 @@ __device__ __forceinline__ void consume_tile(float (&acc)[BN / 2], uint8_t* smem
     for (int k = 0; k < BK / 16; ++k) {
       const uint64_t da = gmma_desc(sA + k * A_KSTEP, A_LBO, 1024);
       const uint32_t scale_d = (kb | k) != 0 ? 1u : 0u;
-      if constexpr (BN == 256 && kHalves256) {
+      if constexpr (BN == 256) {
         // two m64n128 halves (columns 128.. start 16 KB into the B tile, K- or MN-major): an m64n256
         // wgmma needs more than the 128 registers a thread of a 512-thread kernel launches with.
         // The fragment layout, and every output bit, is that of the m64n256 form.
@@ -427,7 +395,7 @@ __device__ __forceinline__ void consume_tile(float (&acc)[BN / 2], uint8_t* smem
       if (kCluster == 2) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[prev]), peer));
     }
     prev = stage;
-    if (++stage == kStages) { stage = 0; phase ^= 1; }
+    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
   }
   wgmma_wait<0>();
   if (releaser) {
@@ -460,7 +428,7 @@ struct WsSmem {
       mbar_init(&empty_bar[s], 2 * kCluster);
     }
     for (int s = 0; s < EPI_CHUNKS; ++s) {
-      mbar_init(&chunk_full[s], EPI_WARPS);
+      mbar_init(&chunk_full[s], CONSUMER_WARPS);
       mbar_init(&chunk_empty[s], 4);
     }
     fence_barrier_init();
@@ -483,7 +451,6 @@ template <int BN, bool A_MN, bool B_MN, bool kBF16, int kCluster, int EPI>
 __global__ void __launch_bounds__(GEMM_WS_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const GemmParams p) {
-  using Cfg = WsCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.  The offset is computed in the shared window
   // and applied by pointer arithmetic on the __shared__ array so that the compiler keeps the
@@ -525,8 +492,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int kb1 = min(num_kb, kb0 + p.kb_per_split);
         const int m0 = (tile / p.tiles_n) * (kCluster * BM) + static_cast<int>(rank) * BM;
         const int n0 = (tile % p.tiles_n) * BN;
-        produce_tile<BN, A_MN, B_MN, kCluster, Cfg::STAGES>(smem, sm.full_bar, sm.empty_bar, &tmA, &tmB, m0, n0,
-                                                            kb0, kb1, stage, phase, rank);
+        produce_tile<BN, A_MN, B_MN, kCluster>(smem, sm.full_bar, sm.empty_bar, &tmA, &tmB, m0, n0,
+                                               kb0, kb1, stage, phase, rank);
       }
     }
   } else if (warp < 12) {
@@ -543,8 +510,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       const int kb0 = (unit / num_tiles) * p.kb_per_split;
       const int kb1 = min(num_kb, kb0 + p.kb_per_split);
       const int n0 = (tile % p.tiles_n) * BN;
-      consume_tile<BN, A_MN, B_MN, kBF16, kCluster, Cfg::STAGES, true>(acc, smem, sm.full_bar, sm.empty_bar,
-                                                                       kb1 - kb0, cw >> 2, stage, phase, rank ^ 1u);
+      consume_tile<BN, A_MN, B_MN, kBF16, kCluster>(acc, smem, sm.full_bar, sm.empty_bar,
+                                                    kb1 - kb0, cw >> 2, stage, phase, rank ^ 1u);
       handoff_tile<BN>(acc, n0, p.N, cw, lane, sm.ring, sm.chunk_full, sm.chunk_empty, cs, cphase);
     }
   } else {
@@ -584,7 +551,6 @@ __device__ __forceinline__ int group_of_tile(const GroupedParams& g, int tile) {
 template <int BN, bool kBF16, int EPI>
 __global__ void __launch_bounds__(GEMM_WS_THREADS, 1)
 gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
-  using Cfg = WsCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const WsSmem<BN> sm(smem);
@@ -609,8 +575,8 @@ gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
         const int lt = tile - g.tile_start[pi];
         const int m0 = (lt / g.tiles_n[pi]) * BM;
         const int n0 = (lt % g.tiles_n[pi]) * BN;
-        produce_tile<BN, true, true, 1, Cfg::STAGES>(smem, sm.full_bar, sm.empty_bar, &tm.a[pi], &tm.b[pi], m0, n0,
-                                                     0, num_kb, stage, phase, 0u);
+        produce_tile<BN, true, true, 1>(smem, sm.full_bar, sm.empty_bar, &tm.a[pi], &tm.b[pi], m0, n0,
+                                        0, num_kb, stage, phase, 0u);
       }
     }
   } else if (warp < 12) {
@@ -625,8 +591,8 @@ gemm_group_kernel(const __grid_constant__ TmPack tm, const GroupedParams g) {
       const int pi = group_of_tile(g, tile);
       const int lt = tile - g.tile_start[pi];
       const int n0 = (lt % g.tiles_n[pi]) * BN;
-      consume_tile<BN, true, true, kBF16, 1, Cfg::STAGES, true>(acc, smem, sm.full_bar, sm.empty_bar, num_kb,
-                                                                cw >> 2, stage, phase, 0u);
+      consume_tile<BN, true, true, kBF16, 1>(acc, smem, sm.full_bar, sm.empty_bar, num_kb,
+                                             cw >> 2, stage, phase, 0u);
       handoff_tile<BN>(acc, n0, g.N[pi], cw, lane, sm.ring, sm.chunk_full, sm.chunk_empty, cs, cphase);
     }
   } else {

@@ -11,8 +11,6 @@
 //   cvt           16-bit <- fp32 (+ optional accumulate): small-gradient finalisation
 // One warp per row; a lane owns the same columns in every row it visits so that the column
 // reductions of ln_bwd stay in registers until one smem + atomic step per CTA.
-#include <stdlib.h>
-
 #include "common.h"
 #include "ptx.cuh"
 
@@ -767,10 +765,7 @@ int launch_ln_bwd(int dtype, const LnBwdParams& p, cudaStream_t stream) {
     return set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
                      LN_MAX_VEC * 256, p.H);
   int grid = (p.rows + 7) / 8;
-  // one wave; UB200_LN_BWD_CTAS_PER_SM (default 1) trades more column-sum atomics for more
-  // rows in flight per SM
-  static const int per_sm = [] { const char* e = getenv("UB200_LN_BWD_CTAS_PER_SM"); int v = e ? atoi(e) : 1; return v < 1 ? 1 : (v > 4 ? 4 : v); }();
-  const int cap = num_sms() * per_sm;
+  const int cap = num_sms();   // one wave
   if (grid > cap) grid = cap;
   ProfScope ps(stream);
   if (dtype == UB200_BF16) UB_CHECK_CUDA(launch_ln_bwd_nv<true>(p, grid, stream));
@@ -899,40 +894,28 @@ extern "C" int ub200_layernorm_bwd(const ub200_ln_bwd_args* a, ub200_stream_t st
   p.rng_dev = reinterpret_cast<const unsigned long long*>(a->rng_offset_dev);
   UB_CHECK_ARG(a->act == UB200_LN_ACT_NONE || a->act == UB200_LN_ACT_RELU, "layernorm_bwd: unknown act %d", a->act);
   const bool relu = a->act == UB200_LN_ACT_RELU;
-  if (relu || p.H > ub::LN_MAX_VEC * 256) {
-    // ReLU rows and rows wider than 1024: always the split form (row kernel + column kernel, fixed-order
-    // in the deterministic mode), on plain rows.  With ReLU, dx_drop receives dpre = dx o (pre > 0).
-    UB_CHECK_ARG(a->stats_ws != nullptr, "layernorm_bwd: ReLU or hidden > %d needs stats_ws (rows x 2 floats)",
-                 ub::LN_MAX_VEC * 256);
-    UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
-    UB_CHECK_ARG(a->row_kind == nullptr && !(a->dropout_on_dy & 1),
-                 "layernorm_bwd: ReLU or hidden > %d takes no row_kind and no dropout on dy", ub::LN_MAX_VEC * 256);
-    if (relu) {
-      UB_CHECK_ARG(a->dx_drop != nullptr, "layernorm_bwd: ReLU needs dx_drop (it receives dpre)");
-      UB_CHECK_ARG(a->dropout_p == 0.f, "layernorm_bwd: ReLU and dropout share dx_drop; dropout_p must be 0");
-      p.dx_drop = a->dx_drop;
-    }
-    if (p.H % 8 != 0 || p.H > ub::LN_WIDE_MAX_VEC * 256 || p.rows <= 0)
-      return ub::set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
-                           ub::LN_WIDE_MAX_VEC * 256, p.H);
-    return ub::launch_ln_bwd_split(a->dtype, p, relu, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
+  // The split form (row kernel + column kernel, fixed-order in the deterministic mode) is the only one
+  // for ReLU rows and rows wider than 1024, the deterministic mode takes it for every case, and
+  // stats_ws selects it for plain rows (no row_kind, no dropout on dy).
+  const bool split_only = relu || p.H > ub::LN_MAX_VEC * 256;
+  const bool plain = a->row_kind == nullptr && !p.dy_drop;
+  if (!(split_only || ub::deterministic() || (a->stats_ws != nullptr && plain)))
+    return ub::launch_ln_bwd(a->dtype, p, reinterpret_cast<cudaStream_t>(stream));
+  UB_CHECK_ARG(a->stats_ws != nullptr,
+               "layernorm_bwd: ReLU, hidden > %d and the deterministic mode need stats_ws (rows x 2 floats)",
+               ub::LN_MAX_VEC * 256);
+  UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
+  UB_CHECK_ARG(!split_only || (a->row_kind == nullptr && !(a->dropout_on_dy & 1)),
+               "layernorm_bwd: ReLU or hidden > %d takes no row_kind and no dropout on dy", ub::LN_MAX_VEC * 256);
+  if (relu) {   // dx_drop receives dpre = dx o (pre > 0)
+    UB_CHECK_ARG(a->dx_drop != nullptr, "layernorm_bwd: ReLU needs dx_drop (it receives dpre)");
+    UB_CHECK_ARG(a->dropout_p == 0.f, "layernorm_bwd: ReLU and dropout share dx_drop; dropout_p must be 0");
+    p.dx_drop = a->dx_drop;
   }
-  if (ub::deterministic()) {   // one form for every case: row kernel + fixed-order column kernel
-    UB_CHECK_ARG(a->stats_ws != nullptr, "layernorm_bwd: deterministic mode needs stats_ws (rows x 2 floats)");
-    UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
-    if (p.H % 8 != 0 || p.H > ub::LN_MAX_VEC * 256 || p.rows <= 0)
-      return ub::set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
-                           ub::LN_MAX_VEC * 256, p.H);
-    return ub::launch_ln_bwd_split(a->dtype, p, false, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
-  }
-  if (a->stats_ws != nullptr && a->row_kind == nullptr && !p.dy_drop) {
-    UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->stats_ws) & 7) == 0, "layernorm_bwd: stats_ws must be 8-byte aligned");
-    if (p.H % 8 != 0 || p.H > ub::LN_MAX_VEC * 256 || p.rows <= 0)
-      return ub::set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
-                           ub::LN_MAX_VEC * 256, p.H);
-    return ub::launch_ln_bwd_split(a->dtype, p, false, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
-  }
-  return ub::launch_ln_bwd(a->dtype, p, reinterpret_cast<cudaStream_t>(stream));
+  if (p.H % 8 != 0 || p.H > ub::LN_WIDE_MAX_VEC * 256 || p.rows <= 0)
+    return ub::set_error(UB200_EUNSUPPORTED, "ln_bwd: need rows > 0, H %% 8 == 0 and H <= %d (H=%d)",
+                         ub::LN_WIDE_MAX_VEC * 256, p.H);
+  return ub::launch_ln_bwd_split(a->dtype, p, relu, a->stats_ws, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int ub200_gather_rows(const void* src, void* dst, const int32_t* index, int32_t rows,

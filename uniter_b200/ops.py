@@ -27,12 +27,10 @@ def _follows_torch(fn):
 def gemm(a, b, *, a_major=0, b_major=0, bias=None, residual=None, aux=None, out=None,
          gelu=False, dgelu=False, accumulate=False, out_fp32=False, colsum=None,
          dropout_p=0.0, rng_seed=0, rng_stream=0, tile_n=0, max_ctas=0, cluster=0, k_splits=0,
-         n_valid=0, rng_offset_dev=None, tanh=False, ln=None, _debug_flags=0):
+         n_valid=0, rng_offset_dev=None, tanh=False):
     """D = epilogue(A . B^T) on the wgmma GEMM core.  Returns `out` (and pre-activation if gelu).
 
     a: [M,K] (a_major=0) or [K,M] (a_major=1);  b: [N,K] (b_major=0) or [K,N] (b_major=1).
-    ln=(gamma, beta): fused residual + LayerNorm epilogue — returns (s, LayerNorm(s)); needs bias and
-    residual, N = 768 or 1024.
     k_splits > 1 (or -1 = fill the SMs): split-K into a zero-initialised fp32 `out` through atomics.
     n_valid: b holds only n_valid of the N (= out.size(1)) output features; the rest get acc = 0.
     """
@@ -80,10 +78,6 @@ def gemm(a, b, *, a_major=0, b_major=0, bias=None, residual=None, aux=None, out=
         epi |= EPI_GELU
     if tanh:
         epi |= _lib.EPI_TANH
-    ln_out = None
-    if ln is not None:
-        epi |= _lib.EPI_LN
-        ln_out = torch.empty(M, N, device=a.device, dtype=a.dtype)
     if dgelu:
         epi |= EPI_DGELU
     if accumulate:
@@ -95,7 +89,6 @@ def gemm(a, b, *, a_major=0, b_major=0, bias=None, residual=None, aux=None, out=
     if splitk:
         assert out.dtype == torch.float32 and epi == EPI_OUT_F32, "split-K: fp32 out, no other epilogue"
         epi |= EPI_ATOMIC
-    epi |= _debug_flags
     args = _lib.GemmArgs(
         a=a.data_ptr(), b=b.data_ptr(), lda=a.stride(0), ldb=b.stride(0),
         a_major=a_major, b_major=b_major, M=M, N=N, K=K,
@@ -107,13 +100,8 @@ def gemm(a, b, *, a_major=0, b_major=0, bias=None, residual=None, aux=None, out=
         ldo=out.stride(0),
         dropout_p=float(dropout_p), rng_seed=int(rng_seed), rng_stream=int(rng_stream),
         tile_n=int(tile_n), max_ctas=int(max_ctas), cluster=int(cluster), k_splits=int(k_splits),
-        n_valid=int(n_valid), rng_offset_dev=rng_offset_dev,
-        ln_gamma=_lib.ptr(ln[0]) if ln is not None else None,
-        ln_beta=_lib.ptr(ln[1]) if ln is not None else None, ln_out=_lib.ptr(ln_out),
-        ldln=ln_out.stride(0) if ln_out is not None else 0)
+        n_valid=int(n_valid), rng_offset_dev=rng_offset_dev)
     _lib.check(lib.ub200_gemm(C.byref(args), _lib.current_stream()))
-    if ln is not None:
-        return out, ln_out
     return (out, out2) if gelu else out
 
 
