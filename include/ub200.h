@@ -462,6 +462,40 @@ int64_t ub200_region_score_workspace_bytes(int32_t batch, int32_t hidden);
 int ub200_region_score_fwd(const ub200_region_score_args* args, ub200_stream_t stream);
 int ub200_region_score_bwd(const ub200_region_score_args* args, ub200_stream_t stream);
 
+/* Word-region alignment (model/ot.py, model/pretrain.py:166-193): the IPOT optimal-transport distance
+ * between the text rows and the region rows of each image-text pair, read straight from the packed
+ * [total_rows, H] 16-bit encoder output.  Pair b owns rows cu_seqlens[b] .. cu_seqlens[b+1] - 1: its
+ * m = txt_len[b] text rows x_i first, then its n regions y_j (int32 device tables).  One CTA per pair.
+ *   x^ = x / max(|x|, 1e-5), y^ likewise (fp32 row norms);  C[i, j] = 1 - x^_i . y^_j, the dot products
+ *   on tensor cores (mma.sync m16n8k16, 16-bit inputs, fp32 accumulation);
+ *   IPOT with beta 0.5, 50 iterations, k = 1 (model/ot.py:36-67): sigma = 1/m, T = 1, A = exp(-C^T/beta);
+ *   each iteration Q = A * T, delta = 1/(n Q sigma), sigma = 1/(m delta^T Q), T = delta * Q * sigma;
+ *   dist[b] = round16(sum_ij C[i, j] T[j, i]), stored as fp32.
+ * C, A and T of a pair stay in shared memory for all 50 iterations; the forward saves T and the row
+ * norms in the workspace.  The backward treats T as a constant: with g = d_dist[b], dC = g T^T, then
+ * dx^ = -dC y^, dy^ = -dC^T x^ and the F.normalize backward give d_packed for every row of every pair;
+ * rows from cu_seqlens[batch] to total_rows - 1 get 0.  Fixed summation orders, no float atomics.
+ * Supported: hidden a multiple of 16 up to 1024, and max_m * max_n <= UB200_WRA_MAX_MN (11 x 1024:
+ * three fp32 [n, m] matrices and four fp32 vectors fit the 227 KB of shared memory of one H100 CTA even
+ * at m + n = m n + 1), UB200_EUNSUPPORTED otherwise.  max_m < 1 or max_n < 1 is UB200_EINVAL.  A pair
+ * outside 1 <= m <= max_m, 1 <= n <= max_n (device values the host does not see) gets dist NaN and a
+ * zero gradient. */
+#define UB200_WRA_MAX_MN 11264
+typedef struct {
+  const void* packed;          /* [total_rows, H] */
+  const int32_t* cu_seqlens;   /* [batch + 1] */
+  const int32_t* txt_len;      /* [batch] */
+  float* dist;                 /* [batch] (forward) */
+  const float* d_dist;         /* [batch] (backward) */
+  void* d_packed;              /* [total_rows, H] (backward) */
+  void* workspace;             /* >= ub200_wra_workspace_bytes: written by the forward, read by the backward */
+  int64_t workspace_bytes;
+  int32_t total_rows, hidden, batch, max_m, max_n, dtype;
+} ub200_wra_args;
+int64_t ub200_wra_workspace_bytes(int32_t batch, int32_t max_m, int32_t max_n);
+int ub200_wra_fwd(const ub200_wra_args* args, ub200_stream_t stream);
+int ub200_wra_bwd(const ub200_wra_args* args, ub200_stream_t stream);
+
 /* Multi-tensor AdamW on fp32 master weights: replaces optim/adamw.py:43-103 (+ the apex O2
  * master-gradient copy, unscale and master->model copy around it, train_vqa.py:152,190-227) and
  * torch.nn.utils.clip_grad_norm_ (train_vqa.py:223-226).  One segment per parameter tensor;

@@ -129,6 +129,16 @@ class RegionScoreArgs(C.Structure):
         ("mode", C.c_int32), ("dtype", C.c_int32), ("margin", C.c_float)]
 
 
+class WraArgs(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("packed", "cu_seqlens", "txt_len", "dist", "d_dist", "d_packed",
+                                          "workspace")] + [
+        ("workspace_bytes", C.c_int64),
+        ("total_rows", C.c_int32), ("hidden", C.c_int32), ("batch", C.c_int32), ("max_m", C.c_int32),
+        ("max_n", C.c_int32), ("dtype", C.c_int32)]
+
+
+WRA_MAX_MN = 11264      # UB200_WRA_MAX_MN
+
 F32 = 2
 _lib = None
 
@@ -224,6 +234,11 @@ def load():
     for name in ("ub200_region_score_fwd", "ub200_region_score_bwd"):
         getattr(lib, name).restype = C.c_int
         getattr(lib, name).argtypes = [C.POINTER(RegionScoreArgs), C.c_void_p]
+    lib.ub200_wra_workspace_bytes.restype = C.c_int64
+    lib.ub200_wra_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    for name in ("ub200_wra_fwd", "ub200_wra_bwd"):
+        getattr(lib, name).restype = C.c_int
+        getattr(lib, name).argtypes = [C.POINTER(WraArgs), C.c_void_p]
     lib.ub200_gather_rows.restype = C.c_int
     lib.ub200_gather_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
     lib.ub200_peer_flags_bytes.restype = C.c_int64

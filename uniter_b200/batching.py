@@ -13,6 +13,9 @@ GPU path run without a single device->host read:
   masked tokens, in the order of the reference's boolean-mask selection, model/pretrain.py:129-133).
 * ``re_collate`` / ``re_eval_collate`` — data/re.py:146-188, :251-295, plus ``re_index`` / ``re_seg``, the
   flat positions of the region rows and each sample's start and count in them (``re_region_index``).
+* ``itm_ot_collate`` — data/itm.py:128-183: ITM pairs with the word-region alignment inputs (``ot_inputs``,
+  uint8 pads), plus ``ot_txt_lens`` (int32 text lengths) and ``ot_pos_index`` / ``ot_neg_index`` (int64
+  positions of the positive / negative pairs), with which the ITM step reads nothing from the device.
 * ``vcr_collate`` / ``vcr_eval_collate`` — data/vcr.py:162-196, :262-300: every question contributes one
   sequence per choice (4 answers; for eval also the 16 rationale sequences), flattened in order.
 * ``DevicePrefetcher`` — data/loader.py:86-141 (side-stream H2D of pinned batches, joined with
@@ -179,6 +182,35 @@ def re_eval_collate(inputs):
      sent_ids) = map(list, zip(*inputs))
     batch = _re_fields(input_ids, img_feats, img_pos_feats, attn_masks, obj_masks)
     batch["tgt_box"], batch["obj_boxes"], batch["sent_ids"] = tgt_box, obj_boxes, sent_ids
+    return batch
+
+
+def _ot_pad(lens, max_len):
+    pad = torch.zeros(len(lens), max_len, dtype=torch.uint8)
+    for i, n in enumerate(lens):
+        pad[i, n:] = 1
+    return pad
+
+
+def itm_ot_collate(inputs):
+    """inputs: list of (input_ids, img_feat, img_pos_feat, attn_masks, target [1]) — data/itm.py:145-183
+    (ItmDataset with itm_ot_lambda > 0).  ot_scatter maps position j < txt_len of pair i to text slot j
+    and j >= txt_len to image slot j - txt_len (data/itm.py:128-135)."""
+    input_ids, img_feats, img_pos_feats, attn_masks, targets = map(list, zip(*inputs))
+    batch = _joint_fields(input_ids, img_feats, img_pos_feats, attn_masks)
+    targets = torch.cat(targets, dim=0)
+    txt_lens, num_bbs = batch["txt_lens"], batch["num_bbs"]
+    joint_len, max_tl = batch["attn_masks"].size(1), max(txt_lens)
+    ot_scatter = torch.arange(0, joint_len, dtype=torch.long).unsqueeze(0).repeat(len(txt_lens), 1)
+    for i, tl in enumerate(txt_lens):
+        ot_scatter[i, tl:] = torch.arange(max_tl, max_tl + joint_len - tl, dtype=torch.long)
+    batch["targets"] = targets
+    batch["ot_inputs"] = {"ot_scatter": ot_scatter, "scatter_max": ot_scatter.max().item(),
+                          "txt_pad": _ot_pad(txt_lens, max_tl), "img_pad": _ot_pad(num_bbs, max(num_bbs))}
+    batch["ot_txt_lens"] = torch.tensor(txt_lens, dtype=torch.int32)
+    t = targets.tolist()
+    batch["ot_pos_index"] = torch.tensor([i for i, v in enumerate(t) if v == 1], dtype=torch.long)
+    batch["ot_neg_index"] = torch.tensor([i for i, v in enumerate(t) if v == 0], dtype=torch.long)
     return batch
 
 

@@ -15,6 +15,9 @@
 //   region_score      referring-expression head (model/re.py:69-90): Linear(H, 1) over each
 //                     sample's region rows, masked_fill, cross-entropy or ranking hinge, and the
 //                     backward with fixed-order weight-gradient sums (no float atomics).
+//   wra               word-region alignment of ITM pre-training (model/ot.py): per image-text pair
+//                     the cosine cost between its text and region rows, 50 IPOT iterations in
+//                     shared memory, the transport distance and its backward (T held constant).
 #include "common.h"
 #include "ptx.cuh"
 
@@ -553,6 +556,277 @@ region_score_wsum_kernel(const float* __restrict__ part_w, int batch, int H, flo
   if (c < H) dw[c] = s; else if (db != nullptr) db[0] = s;
 }
 
+// ------------------------------------------------------------------------------ word-region alignment
+// model/ot.py:optimal_transport_dist with its defaults (beta 0.5, 50 iterations, k = 1), restricted to the
+// valid n x m block of each pair: the reference's padded entries of A and T are zero, so its 1e4 padding
+// terms never reach a valid entry.  Matrices are [n, m] (region-major, like the reference's T), entry
+// e = j * m + i.
+constexpr int WRA_THREADS = 256;
+constexpr int WRA_ITERS = 50;
+constexpr float WRA_BETA = 0.5f;
+constexpr float WRA_EPS = 1e-5f;   // F.normalize eps of cost_matrix_cosine
+constexpr int WRA_MAXV = 4;        // 16-byte vectors per lane of a row: hidden <= 32 * 8 * 4
+
+// workspace of pair b: T [max_m * max_n] then the raw row norms [max_m + max_n] (text, then regions)
+__device__ __forceinline__ float* wra_pair_ws(const ub200_wra_args& a, int b) {
+  const long long stride = static_cast<long long>(a.max_m) * a.max_n + a.max_m + a.max_n;
+  return reinterpret_cast<float*>(a.workspace) + b * stride;
+}
+
+__device__ __forceinline__ bool wra_pair_ok(const ub200_wra_args& a, int m, int n) {
+  return m >= 1 && n >= 1 && m <= a.max_m && n <= a.max_n;
+}
+
+// D += A (16x16, row) . B (16x8, col), 16-bit inputs, fp32 accumulation
+template <bool kBF16>
+__device__ __forceinline__ void mma_16816(float* d, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                          uint32_t b0, uint32_t b1) {
+  if constexpr (kBF16)
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+                 "{%0,%1,%2,%3};\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+                 "{%0,%1,%2,%3};\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// Shared memory: C, A, P [max_m * max_n] (P holds Q, then T), sigma [max_m], delta [max_n], norms
+// [max_m + max_n], column partials [256] (S * m <= 256 where S > 1).
+template <bool kBF16>
+__global__ void __launch_bounds__(WRA_THREADS)
+wra_fwd_kernel(const ub200_wra_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  using T16 = typename Elem<kBF16>::T;
+  extern __shared__ float wra_sm[];
+  __shared__ float red[8];
+  const int b = blockIdx.x, H = a.hidden, MN = a.max_m * a.max_n;
+  const int start = a.cu_seqlens[b], m = a.txt_len[b], n = a.cu_seqlens[b + 1] - start - m;
+  if (!wra_pair_ok(a, m, n)) {
+    if (threadIdx.x == 0) a.dist[b] = __int_as_float(0x7fc00000);
+    return;
+  }
+  float* C = wra_sm;
+  float* A = C + MN;
+  float* P = A + MN;
+  float* sig = P + MN;
+  float* del = sig + a.max_m;
+  float* nrm = del + a.max_n;
+  float* part = nrm + a.max_m + a.max_n;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, mn = m * n;
+  const T16* X = reinterpret_cast<const T16*>(a.packed) + static_cast<long long>(start) * H;
+  const T16* Y = X + static_cast<long long>(m) * H;
+
+  // raw row norms in fp32: one warp per row, lane-strided 16-byte vectors, a fixed xor tree
+  for (int r = warp; r < m + n; r += WRA_THREADS / 32) {
+    const uint4* v = reinterpret_cast<const uint4*>(X + static_cast<long long>(r) * H);
+    float s = 0.f;
+    for (int c = lane; c < (H >> 3); c += 32) {
+      float f[8];
+      h_unpack8<kBF16>(__ldg(v + c), f);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) s = fmaf(f[e], f[e], s);
+    }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) nrm[r] = sqrtf(s);
+  }
+  // x_i . y_j: one warp per 16 x 8 tile, fragments loaded straight from global memory; rows past m / n
+  // are clamped to the last valid row and their results dropped
+  {
+    const int g = lane >> 2, t4 = lane & 3, mb = (m + 15) >> 4, nb = (n + 7) >> 3;
+    for (int tile = warp; tile < mb * nb; tile += WRA_THREADS / 32) {
+      const int i0 = (tile / nb) * 16, j0 = (tile % nb) * 8;
+      const uint32_t* xa = reinterpret_cast<const uint32_t*>(X + static_cast<long long>(min(i0 + g, m - 1)) * H) + t4;
+      const uint32_t* xb = reinterpret_cast<const uint32_t*>(X + static_cast<long long>(min(i0 + g + 8, m - 1)) * H) + t4;
+      const uint32_t* yb = reinterpret_cast<const uint32_t*>(Y + static_cast<long long>(min(j0 + g, n - 1)) * H) + t4;
+      float d[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int k = 0; k < (H >> 1); k += 8)
+        mma_16816<kBF16>(d, __ldg(xa + k), __ldg(xb + k), __ldg(xa + k + 4), __ldg(xb + k + 4), __ldg(yb + k),
+                         __ldg(yb + k + 4));
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int i = i0 + g + (q >> 1) * 8, j = j0 + 2 * t4 + (q & 1);
+        if (i < m && j < n) C[j * m + i] = d[q];
+      }
+    }
+  }
+  __syncthreads();
+  for (int e = tid; e < mn; e += WRA_THREADS) {
+    const int j = e / m, i = e - j * m;
+    const float c = 1.f - C[e] * __frcp_rn(fmaxf(nrm[i], WRA_EPS) * fmaxf(nrm[m + j], WRA_EPS));
+    C[e] = c;
+    A[e] = expf(-c / WRA_BETA);
+  }
+  for (int i = tid; i < m; i += WRA_THREADS) sig[i] = __frcp_rn(static_cast<float>(m));
+  __syncthreads();
+
+  // IPOT.  T = delta * Q * sigma of one iteration is folded into the next one's Q = A * T (the same
+  // products in the same order as the two steps).  sigma's column sums run over `S` slices of the
+  // regions, added in slice order.
+  const float fm = static_cast<float>(m), fn = static_cast<float>(n);
+  const int S = m < WRA_THREADS ? WRA_THREADS / m : 1, jper = (n + S - 1) / S;
+  for (int it = 0; it < WRA_ITERS; ++it) {
+    for (int j = warp; j < n; j += WRA_THREADS / 32) {
+      float s = 0.f;
+      for (int i = lane; i < m; i += 32) {
+        const int e = j * m + i;
+        const float q = it == 0 ? A[e] : A[e] * (del[j] * P[e] * sig[i]);
+        P[e] = q;
+        s = fmaf(q, sig[i], s);
+      }
+#pragma unroll
+      for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      __syncwarp();
+      if (lane == 0) del[j] = __frcp_rn(fn * s);
+    }
+    __syncthreads();
+    for (int c = tid; c < S * m; c += WRA_THREADS) {
+      const int sl = c / m, i = c - sl * m;
+      float s = 0.f;
+      for (int j = sl * jper; j < min(n, (sl + 1) * jper); ++j) s = fmaf(del[j], P[j * m + i], s);
+      if (S == 1) sig[i] = __frcp_rn(fm * s);
+      else part[c] = s;
+    }
+    __syncthreads();
+    if (S > 1) {
+      for (int i = tid; i < m; i += WRA_THREADS) {
+        float s = part[i];
+        for (int sl = 1; sl < S; ++sl) s += part[sl * m + i];
+        sig[i] = __frcp_rn(fm * s);
+      }
+      __syncthreads();
+    }
+  }
+  float* ws = wra_pair_ws(a, b);
+  float dist = 0.f;
+  for (int e = tid; e < mn; e += WRA_THREADS) {
+    const int j = e / m, i = e - j * m;
+    const float t = del[j] * P[e] * sig[i];
+    ws[e] = t;
+    dist = fmaf(C[e], t, dist);
+  }
+  for (int r = tid; r < m + n; r += WRA_THREADS) ws[MN + r] = nrm[r];
+  dist = block_sum(dist, red);
+  if (tid == 0) a.dist[b] = Elem<kBF16>::to_f(Elem<kBF16>::from_f(dist));
+}
+
+// One output row pair per warp iteration: d(own row) = normalize-backward(-g sum_k w_k other_k), with
+// w_k = T[k, i] / |y_k| for a text row i (other = regions) and T[j, k] / |x_k| for a region row j.
+template <bool kBF16>
+__device__ __forceinline__ void wra_bwd_rows(const ub200_wra_args& a, const float* P, const float* nrm, int m,
+                                             int n, const typename Elem<kBF16>::T* X, bool text, int o0,
+                                             float g, typename Elem<kBF16>::T* dX) {
+  using T16 = typename Elem<kBF16>::T;
+  const int H = a.hidden, lane = threadIdx.x & 31, nvec = H >> 3;
+  const int own_n = text ? m : n, K = text ? n : m;
+  const T16* own = text ? X : X + static_cast<long long>(m) * H;
+  const T16* other = text ? X + static_cast<long long>(m) * H : X;
+  const float* onrm = text ? nrm + m : nrm;
+  const bool two = o0 + 1 < own_n;
+  float acc[2][WRA_MAXV][8];
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int v = 0; v < WRA_MAXV; ++v)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[r][v][e] = 0.f;
+  for (int k = 0; k < K; ++k) {
+    const float inv = __frcp_rn(fmaxf(onrm[k], WRA_EPS));
+    const float w0 = (text ? P[k * m + o0] : P[o0 * m + k]) * inv;
+    const float w1 = two ? (text ? P[k * m + o0 + 1] : P[(o0 + 1) * m + k]) * inv : 0.f;
+    const uint4* ov = reinterpret_cast<const uint4*>(other + static_cast<long long>(k) * H);
+#pragma unroll
+    for (int v = 0; v < WRA_MAXV; ++v) {
+      if (lane + 32 * v < nvec) {
+        float f[8];
+        h_unpack8<kBF16>(__ldg(ov + lane + 32 * v), f);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          acc[0][v][e] = fmaf(w0, f[e], acc[0][v][e]);
+          acc[1][v][e] = fmaf(w1, f[e], acc[1][v][e]);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    if (r == 1 && !two) break;
+    const int o = o0 + r;
+    const float nr = (text ? nrm : nrm + m)[o], s = fmaxf(nr, WRA_EPS), inv = __frcp_rn(s);
+    const uint4* xv = reinterpret_cast<const uint4*>(own + static_cast<long long>(o) * H);
+    float xs[WRA_MAXV][8];
+    float dot = 0.f;
+#pragma unroll
+    for (int v = 0; v < WRA_MAXV; ++v) {
+      if (lane + 32 * v < nvec) {
+        h_unpack8<kBF16>(__ldg(xv + lane + 32 * v), xs[v]);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          acc[r][v][e] *= -g;                          // d(x^) = -g sum_k w_k other_k
+          dot = fmaf(acc[r][v][e], xs[v][e], dot);
+        }
+      }
+    }
+#pragma unroll
+    for (int q = 16; q >= 1; q >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, q);
+    // x / max(|x|, eps): the norm's gradient flows only where |x| >= eps (clamp_min)
+    const float coef = nr >= WRA_EPS ? dot / (s * s * s) : 0.f;
+    uint4* dv = reinterpret_cast<uint4*>((text ? dX : dX + static_cast<long long>(m) * H) +
+                                         static_cast<long long>(o) * H);
+#pragma unroll
+    for (int v = 0; v < WRA_MAXV; ++v) {
+      if (lane + 32 * v < nvec) {
+        float out[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) out[e] = acc[r][v][e] * inv - coef * xs[v][e];
+        dv[lane + 32 * v] = h_pack8<kBF16>(out);
+      }
+    }
+  }
+}
+
+// Shared memory: T [max_m * max_n] and the norms [max_m + max_n] of the pair.  Rows from
+// cu_seqlens[batch] on are zeroed by the last CTA.
+template <bool kBF16>
+__global__ void __launch_bounds__(WRA_THREADS)
+wra_bwd_kernel(const ub200_wra_args a) {
+  pdl_launch_dependents();
+  pdl_wait();
+  using T16 = typename Elem<kBF16>::T;
+  extern __shared__ float wra_sm[];
+  const int b = blockIdx.x, H = a.hidden, MN = a.max_m * a.max_n, nvec = H >> 3;
+  const int start = a.cu_seqlens[b], end = a.cu_seqlens[b + 1], m = a.txt_len[b], n = end - start - m;
+  const int tid = threadIdx.x, warp = tid >> 5;
+  T16* dX = reinterpret_cast<T16*>(a.d_packed) + static_cast<long long>(start) * H;
+  const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+  if (b == a.batch - 1)
+    for (long long i = static_cast<long long>(end) * nvec + tid; i < static_cast<long long>(a.total_rows) * nvec;
+         i += WRA_THREADS)
+      reinterpret_cast<uint4*>(a.d_packed)[i] = zero;
+  if (!wra_pair_ok(a, m, n)) {
+    for (long long i = tid; i < static_cast<long long>(max(end - start, 0)) * nvec; i += WRA_THREADS)
+      reinterpret_cast<uint4*>(dX)[i] = zero;
+    return;
+  }
+  float* P = wra_sm;
+  float* nrm = P + MN;
+  const float* ws = wra_pair_ws(a, b);
+  for (int e = tid; e < m * n; e += WRA_THREADS) P[e] = ws[e];
+  for (int r = tid; r < m + n; r += WRA_THREADS) nrm[r] = ws[MN + r];
+  __syncthreads();
+  const float g = a.d_dist[b];
+  const T16* X = reinterpret_cast<const T16*>(a.packed) + static_cast<long long>(start) * H;
+  const int mu = (m + 1) >> 1, nu = (n + 1) >> 1;
+  for (int u = warp; u < mu + nu; u += WRA_THREADS / 32) {
+    if (u < mu) wra_bwd_rows<kBF16>(a, P, nrm, m, n, X, true, 2 * u, g, dX);
+    else wra_bwd_rows<kBF16>(a, P, nrm, m, n, X, false, 2 * (u - mu), g, dX);
+  }
+}
+
 }  // namespace ub
 
 // ------------------------------------------------------------------------------ C ABI
@@ -815,4 +1089,66 @@ extern "C" int ub200_region_score_bwd(const ub200_region_score_args* a, ub200_st
   UB_CHECK_CUDA(launch_pdl(region_score_wsum_kernel, dim3(grid), dim3(RE_THREADS), 0, stream, 1,
                            static_cast<const float*>(a->workspace), a->batch, a->hidden, a->dweight, a->dbias));
   return 0;
+}
+
+// ------------------------------------------------------------------------------ word-region alignment
+extern "C" int64_t ub200_wra_workspace_bytes(int32_t batch, int32_t max_m, int32_t max_n) {
+  if (batch <= 0 || max_m <= 0 || max_n <= 0) return 0;
+  return static_cast<int64_t>(batch) * (static_cast<int64_t>(max_m) * max_n + max_m + max_n) * 4;
+}
+
+static int wra_check(const ub200_wra_args* a, const char* who) {
+  using namespace ub;
+  UB_CHECK_ARG(a && a->packed && a->cu_seqlens && a->txt_len && a->workspace, "%s: null pointer", who);
+  UB_CHECK_ARG(a->batch > 0 && a->total_rows >= 0 && a->max_m >= 1 && a->max_n >= 1,
+               "%s: need batch > 0, total_rows >= 0, max_m >= 1 and max_n >= 1", who);
+  UB_CHECK_ARG(a->dtype == UB200_F16 || a->dtype == UB200_BF16, "%s: dtype must be F16 or BF16", who);
+  UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->packed) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->workspace) & 15) == 0,
+               "%s: packed and workspace must be 16-byte aligned", who);
+  UB_CHECK_ARG(a->workspace_bytes >= ub200_wra_workspace_bytes(a->batch, a->max_m, a->max_n),
+               "%s: workspace of %lld bytes, %lld needed", who, (long long)a->workspace_bytes,
+               (long long)ub200_wra_workspace_bytes(a->batch, a->max_m, a->max_n));
+  if (a->hidden <= 0 || a->hidden % 16 != 0 || a->hidden > 32 * 8 * WRA_MAXV)
+    return set_error(UB200_EUNSUPPORTED, "%s: hidden %d is not a multiple of 16 up to %d", who, a->hidden,
+                     32 * 8 * WRA_MAXV);
+  if (static_cast<long long>(a->max_m) * a->max_n > UB200_WRA_MAX_MN)
+    return set_error(UB200_EUNSUPPORTED, "%s: max_m * max_n = %d * %d exceeds %d", who, a->max_m, a->max_n,
+                     UB200_WRA_MAX_MN);
+  return 0;
+}
+
+template <typename K>
+static int wra_launch(K kern, unsigned long long& configured, size_t smem, const ub200_wra_args* a,
+                      cudaStream_t stream) {
+  using namespace ub;
+  if (first_use_on_device(configured))
+    UB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(4 * (5 * UB200_WRA_MAX_MN + 2 + WRA_THREADS))));
+  ProfScope ps(stream);
+  UB_CHECK_CUDA(launch_pdl(kern, dim3(a->batch), dim3(WRA_THREADS), smem, stream, 1, *a));
+  return 0;
+}
+
+extern "C" int ub200_wra_fwd(const ub200_wra_args* a, ub200_stream_t stream_) {
+  using namespace ub;
+  if (int rc = wra_check(a, "wra_fwd")) return rc;
+  UB_CHECK_ARG(a->dist, "wra_fwd: null dist");
+  static unsigned long long cfg[2];
+  const size_t mn = static_cast<size_t>(a->max_m) * a->max_n;
+  const size_t smem = 4 * (3 * mn + 2 * (static_cast<size_t>(a->max_m) + a->max_n) + WRA_THREADS);
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (a->dtype == UB200_BF16) return wra_launch(wra_fwd_kernel<true>, cfg[1], smem, a, stream);
+  return wra_launch(wra_fwd_kernel<false>, cfg[0], smem, a, stream);
+}
+
+extern "C" int ub200_wra_bwd(const ub200_wra_args* a, ub200_stream_t stream_) {
+  using namespace ub;
+  if (int rc = wra_check(a, "wra_bwd")) return rc;
+  UB_CHECK_ARG(a->d_dist && a->d_packed, "wra_bwd: null pointer");
+  UB_CHECK_ARG((reinterpret_cast<uintptr_t>(a->d_packed) & 15) == 0, "wra_bwd: d_packed must be 16-byte aligned");
+  static unsigned long long cfg[2];
+  const size_t smem = 4 * (static_cast<size_t>(a->max_m) * a->max_n + a->max_m + a->max_n);
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (a->dtype == UB200_BF16) return wra_launch(wra_bwd_kernel<true>, cfg[1], smem, a, stream);
+  return wra_launch(wra_bwd_kernel<false>, cfg[0], smem, a, stream);
 }

@@ -281,16 +281,47 @@ def _masked_rows(packed, meta, mask2d, index):
     return gather_packed_rows(packed, meta["unpack_ext"][index])
 
 
+class _WraDist(torch.autograd.Function):
+    """Word-region alignment distance of every pair (model/ot.py:optimal_transport_dist over the pair's
+    text and region rows, rounded to the encoder's 16-bit type like `.to(txt_emb)`) in one kernel per
+    direction (ub200_wra_*).  The transport plan is a constant for autograd; the backward writes one
+    gradient row per packed row, zero on the rows of the padding sequence."""
+
+    @staticmethod
+    @_lib.forward_in_mode()
+    def forward(ctx, packed, cu_seqlens, txt_len, batch, max_m, max_n):
+        ws = ops.wra_workspace(batch, max_m, max_n, packed.device)
+        dist = ops.wra_fwd(packed, cu_seqlens, txt_len, batch, max_m, max_n, ws)
+        ctx.save_for_backward(packed, cu_seqlens, txt_len, ws)
+        ctx.shape = (batch, max_m, max_n)
+        return dist.to(packed.dtype)
+
+    @staticmethod
+    @_lib.backward_in_mode
+    def backward(ctx, d_dist):
+        packed, cu_seqlens, txt_len, ws = ctx.saved_tensors
+        d_packed = ops.wra_bwd(packed, cu_seqlens, txt_len, *ctx.shape, ws, d_dist.float().contiguous())
+        return d_packed, None, None, None, None, None
+
+
 class UniterForPretraining(UniterPreTrainedModel):
     """model/pretrain.py:50-229 with every head on libub200: MLM (fused head + cross-entropy), MRFR,
     MRC / MRC-kl (LibTransform + LibLinear over the masked REGION rows gathered straight from the
     packed encoder output) and ITM (library pooler + LibLinear).  Same parameter names, weight tying
     (cls.predictions.decoder <-> word_embeddings, feat_regress.weight <-> img_linear.weight) and
-    forward(batch, task, compute_loss) contract; the OT term of ITM (model/ot.py) is outside the hot
-    path and not implemented (ot_inputs must be None).
+    forward(batch, task, compute_loss) contract.  ITM with `ot_inputs` (data/itm.py:itm_ot_collate) adds
+    word-region alignment (model/pretrain.py:166-193): the IPOT distance between each pair's text rows
+    and region rows, read straight from the packed encoder output (_WraDist, ub200_wra_*), returned as
+    (itm_loss or itm_scores, (ot_pos, ot_neg)).  `ot_scatter` / `scatter_max` are not read; the pads may
+    be uint8 or bool.
 
     Fixed-shape (CUDA-graph friendly) variants of the reference's data-dependent row selections are
-    taken from the batch when the loader provides them: `mlm_index` / `mlm_targets`, `mrm_index`."""
+    taken from the batch when the loader provides them: `mlm_index` / `mlm_targets`, `mrm_index`, and for
+    WRA `ot_txt_lens` (int32 [B] text lengths) with `ot_pos_index` / `ot_neg_index` (int64 positions of
+    the positive / negative pairs).  With those the ITM step reads nothing from the device; without them
+    the text lengths come from one read of the pads and ot_pos / ot_neg from masked_select, as the
+    reference reads them.  Where `txt_lens` / `num_bbs` are known on the host, a pair whose text and
+    region counts do not add up to its valid tokens is a ValueError before any launch."""
 
     def __init__(self, config, img_dim, img_label_dim):
         super().__init__(config)
@@ -342,17 +373,53 @@ class UniterForPretraining(UniterPreTrainedModel):
                               reduction="none")
         return prediction_feat
 
+    def _wra_lengths(self, batch, ot_inputs):
+        """(int32 text lengths on the device, max_m, max_n) of the WRA pairs, checked on the host where
+        the lengths are known there.  max_m / max_n are the padded text and region extents."""
+        max_m, max_n = batch["input_ids"].size(1), batch["img_feat"].size(1)
+        if max_m * max_n > _lib.WRA_MAX_MN:
+            raise ValueError("word-region alignment supports max text length x max regions <= %d, got %d x %d"
+                             % (_lib.WRA_MAX_MN, max_m, max_n))
+        dev = batch["attn_masks"].device
+        txt_lens, num_bbs, txt_len = batch["txt_lens"], batch["num_bbs"], batch["ot_txt_lens"]
+        if txt_len is None and (txt_lens is None or num_bbs is None):
+            txt_pad, img_pad = ot_inputs["txt_pad"], ot_inputs["img_pad"]
+            counts = torch.cat([txt_pad.size(1) - (txt_pad != 0).sum(1),
+                                img_pad.size(1) - (img_pad != 0).sum(1)]).tolist()     # one device read
+            txt_lens, num_bbs = counts[:txt_pad.size(0)], counts[txt_pad.size(0):]
+        if txt_lens is not None and num_bbs is not None:
+            seq = self.uniter._pack_meta(batch["attn_masks"])["lens_host"]
+            for b, (m, n) in enumerate(zip(txt_lens, num_bbs)):
+                if not (1 <= m <= max_m and 1 <= n <= max_n) or (seq is not None and m + n != seq[b]):
+                    raise ValueError("pair %d: %d text tokens and %d regions do not fill its %s valid tokens "
+                                     "(padded extents %d x %d)" % (b, m, n, seq[b] if seq else "?", max_m, max_n))
+        if txt_len is None:
+            txt_len = torch.tensor(list(txt_lens), dtype=torch.int32)
+        return txt_len.to(dev, torch.int32).contiguous(), max_m, max_n
+
     def forward_itm(self, batch, compute_loss=True):                      # model/pretrain.py:156-199
-        if batch["ot_inputs"] is not None:
-            raise NotImplementedError("the OT / WRA term (model/ot.py) is outside the hot path")
+        ot_inputs = batch["ot_inputs"]
+        if ot_inputs is not None:
+            txt_len, max_m, max_n = self._wra_lengths(batch, ot_inputs)
         packed, meta = self._encode(batch)
         B, L = meta["n_batch"], meta["L"]
         cls_rows = meta["unpack_ext"][::L][:B]          # packed row of position (b, 0): the [CLS] token
         pooled = self.uniter.pooler(gather_packed_rows(packed, cls_rows.contiguous()))
         itm_scores = LibLinear.apply(pooled, self.itm_output.weight, self.itm_output.bias, False, False)
+        ot_loss = None
+        if ot_inputs is not None:
+            # the pairs' text rows then region rows, in the packed layout of the prefix masks
+            ot_dist = _WraDist.apply(packed, meta["cu_seqlens"], txt_len, B, max_m, max_n)
+            targets = batch["targets"]
+            if batch["ot_pos_index"] is not None and batch["ot_neg_index"] is not None:
+                dev = ot_dist.device
+                ot_loss = (ot_dist.index_select(0, batch["ot_pos_index"].to(dev)),
+                           ot_dist.index_select(0, batch["ot_neg_index"].to(dev)))
+            else:
+                ot_loss = (ot_dist.masked_select(targets == 1), ot_dist.masked_select(targets == 0))
         if compute_loss:
-            return F.cross_entropy(itm_scores.float(), batch["targets"], reduction="none"), None
-        return itm_scores, None
+            return F.cross_entropy(itm_scores.float(), batch["targets"], reduction="none"), ot_loss
+        return itm_scores, ot_loss
 
     def forward_mrc(self, batch, task, compute_loss=True):                # model/pretrain.py:201-229
         packed, meta = self._encode(batch, img_masks=batch["img_masks"])

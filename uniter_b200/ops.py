@@ -348,6 +348,50 @@ def region_score_bwd(rows, weight, seg, obj_masks, targets, scores, lse, neg, dl
     return d_rows, dw, db
 
 
+def _wra_args(packed, cu_seqlens, txt_len, batch, max_m, max_n, workspace):
+    assert packed.dim() == 2 and packed.is_contiguous()
+    assert cu_seqlens.dtype == torch.int32 and cu_seqlens.numel() >= batch + 1
+    assert txt_len.dtype == torch.int32 and txt_len.is_contiguous() and txt_len.numel() == batch
+    assert workspace.dtype == torch.float32 and workspace.is_contiguous()
+    return _lib.WraArgs(
+        packed=packed.data_ptr(), cu_seqlens=cu_seqlens.data_ptr(), txt_len=txt_len.data_ptr(),
+        workspace=workspace.data_ptr(), workspace_bytes=workspace.numel() * 4, total_rows=packed.size(0),
+        hidden=packed.size(1), batch=batch, max_m=int(max_m), max_n=int(max_n), dtype=_lib.dtype_code(packed.dtype))
+
+
+def wra_workspace(batch, max_m, max_n, device):
+    """fp32 workspace of ub200_wra_fwd / _bwd: the transport plans and row norms of every pair."""
+    return torch.empty(_lib.load().ub200_wra_workspace_bytes(batch, max_m, max_n) // 4, device=device,
+                       dtype=torch.float32)
+
+
+@_follows_torch
+def wra_fwd(packed, cu_seqlens, txt_len, batch, max_m, max_n, workspace):
+    """Word-region alignment distance [batch] (fp32 holding 16-bit-rounded values) of the pairs of the
+    packed encoder output [T_pad, H]: pair b owns rows cu_seqlens[b] .. cu_seqlens[b+1] - 1, its txt_len[b]
+    text rows first.  max_m / max_n bound every pair's text / region count.  Writes the plans and norms
+    the backward reads into `workspace` (wra_workspace)."""
+    lib = _lib.load()
+    a = _wra_args(packed, cu_seqlens, txt_len, batch, max_m, max_n, workspace)
+    dist = torch.empty(batch, device=packed.device, dtype=torch.float32)
+    a.dist = dist.data_ptr()
+    _lib.check(lib.ub200_wra_fwd(C.byref(a), _lib.current_stream()))
+    return dist
+
+
+@_follows_torch
+def wra_bwd(packed, cu_seqlens, txt_len, batch, max_m, max_n, workspace, d_dist):
+    """Backward of wra_fwd with its plans held constant: d_packed [T_pad, H] 16-bit, zero on rows from
+    cu_seqlens[batch] on."""
+    lib = _lib.load()
+    a = _wra_args(packed, cu_seqlens, txt_len, batch, max_m, max_n, workspace)
+    assert d_dist.dtype == torch.float32 and d_dist.is_contiguous() and d_dist.numel() == batch
+    d_packed = torch.empty_like(packed)
+    a.d_dist, a.d_packed = d_dist.data_ptr(), d_packed.data_ptr()
+    _lib.check(lib.ub200_wra_bwd(C.byref(a), _lib.current_stream()))
+    return d_packed
+
+
 @_follows_torch
 def gather_rows(src, index, rows=None):
     """dst[r] = src[index[r]] if index[r] >= 0 else 0 (int32 index; bit-exact row mover)."""
